@@ -112,7 +112,11 @@ B200_API int b200_ctx_timer_stop(b200_ctx *ctx, float *ms);
 B200_API int b200_ctx_profile_enable(b200_ctx *ctx, int on);
 B200_API int b200_ctx_profile_read(b200_ctx *ctx, int slot, double *total_ms, int64_t *launches, int reset);
 /* Tuning knobs (do not change results beyond floating-point summation order):
- *   "spmv_kernel": 0 = auto, 1 = sub-warp-per-row kernel, 2 = TMA-streamed kernel (when the tiles fit)
+ *   "spmv_kernel": 0 = auto (band stream for operators that have a band description, see b200_csr_stream_kind,
+ *           else the CSR stream when the tiles fit, else sub-warp per row), 1 = sub-warp-per-row kernel,
+ *           2 = TMA-streamed CSR kernel (when the tiles fit), 3 = band stream (when the operator has a band
+ *           description and x is 16-byte aligned, else as 0).  The band stream and the CSR stream give
+ *           bit-identical results
  *   "snake": 1 (default) = consecutive hot kernels of a solver sweep the rows in alternating directions so
  *           that each starts on the data the previous one touched last (L2 reuse); 0 = always ascending
  *   "orth_fused": 1 (default) = orthogonalize_and_normalize! (CGS / DGKS) is ONE cooperative launch (dots, update, norm,
@@ -175,6 +179,12 @@ B200_API int b200_csr_info(const b200_csr *A, int64_t *m_local, int64_t *n_globa
  * (real element types: adjoint == transpose).  Single-GPU contexts; on multi-GPU contexts pass the row slabs of A'
  * to b200_csr_from_csr_slab. */
 B200_API int b200_csr_transpose(b200_ctx *ctx, const b200_csr *A, b200_csr **out);
+/* Which form of the streamed SpMV the operator got when it was built (the form "spmv_kernel" = 0 selects):
+ * kind 3 = band stream (a single-GPU operator whose 512-row tiles each have at most 8 distinct diagonal offsets
+ * col - row and whose rows have strictly ascending columns: per tile its offsets, per row one mask byte),
+ * 2 = CSR stream, 1 = sub-warp-per-row kernel.  structure_bytes = bytes of structure (everything but vals and the
+ * vectors) that form reads per SpMV: 576 per 512-row tile for the band stream, 4*nnz + 4*(rows+1) for CSR. */
+B200_API int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes);
 /* diag(A) of the local rows into a device vector (JacobiPrec(diag(A)), reference test/cg.jl:57) */
 B200_API int b200_csr_diag(b200_ctx *ctx, const b200_csr *A, void *diag_dev);
 /* device CSR arrays back to the host (tests) */

@@ -285,6 +285,24 @@ __global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
     cg_finish(FIN_DOT, s, total, nullptr, cm);
 }
 
+// K2, band-streamed form (single GPU, operators with a band description): same result contract
+template <typename T>
+__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
+    k_cg_spmv_dot_band(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ u, int64_t m,
+                       T *__restrict__ c, CgScal *s, double *partials, unsigned int *ticket, Comm cm) {
+  pdl_wait();
+  if (s->done) return;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ double red[kStreamThreads / 32];
+  CgDotEpi<T> epi{c, u, 0.0};
+  spmv_band_tiles<T>(ba, vals, u, m, m, epi, reinterpret_cast<BandSmem<T> *>(smem_raw), cm.rev != 0);
+  pdl_launch_dependents();
+  const double acc = block_sum<kStreamThreads>(epi.acc, red);
+  double total;
+  if (grid_reduce_finish<kStreamThreads>(acc, partials, ticket, red, &total) && threadIdx.x < 32)
+    cg_finish(FIN_DOT, s, total, nullptr, cm);
+}
+
 // K3: r -= alpha*c ; ||r||^2   (x += alpha*u is applied by the next K1 / k_cg_flush_x)
 template <typename T>
 __global__ void __launch_bounds__(kThreads) k_cg_update_r(T *__restrict__ r, const T *__restrict__ c, int64_t n,
@@ -548,7 +566,15 @@ struct CgEngine {
     }
     XView<T> xv = make_xview<T>(A, u, peer && !fold_halo);
     const Comm cm = comm(!fold_halo, next_sweep());
-    if (use_stream(ctx, A)) {
+    if (use_band(ctx, A, u)) {
+      const int grid = stream_grid_size(ctx, A);
+      const size_t smem = sizeof(BandSmem<T>);
+      ProfScope prof(ctx, 0);
+      B200_SMEM_ATTR_ONCE(ctx, smem, k_cg_spmv_dot_band<T>);
+      B200_CUDA(launch_chained(ctx->opt_pdl != 0, k_cg_spmv_dot_band<T>, dim3(grid), dim3(kStreamThreads), smem,
+                               ctx->stream, make_band_args(A), (const T *)A->vals, (const T *)u, n, c, s,
+                               ctx->red.partials, ctx->red.ticket, cm));
+    } else if (use_stream(ctx, A)) {
       const int grid = stream_grid_size(ctx, A);
       const size_t smem = sizeof(StreamSmem<T>);
       ProfScope prof(ctx, 0);

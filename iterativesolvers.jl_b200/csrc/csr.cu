@@ -322,6 +322,88 @@ __global__ void k_tile_max(const int *__restrict__ rowptr, int64_t m, int R, int
   if ((threadIdx.x & 31) == 0) atomicMax(out, local);
 }
 
+// Band description (csr.cuh, spmv_stream.cuh): one block per tile of R = kBandTileRows rows, two rows per thread (r0+lt,
+// r0+lt+R/2).  The tile's distinct offsets come out in ascending order from rounds of "smallest offset above the previous
+// one" (a block minimum); each round also sets that offset's bit in the masks of the rows that have it.  A ninth offset,
+// a row of more than 8 nonzeros or a row whose columns do not strictly ascend sets *bad: the operator keeps the CSR stream.
+constexpr int kBandBuildThreads = kBandTileRows / 2;
+__global__ void __launch_bounds__(kBandBuildThreads)
+    k_band_build(const int *__restrict__ rowptr, const int *__restrict__ colind, int64_t m,
+                 b200_band_tile *__restrict__ hdr, uint8_t *__restrict__ mask, int *bad) {
+  constexpr int R = kBandTileRows, H = kBandBuildThreads;
+  static_assert(2 * H == R, "two rows per thread");
+  __shared__ int red[2][H / 32];
+  const int lt = threadIdx.x, lane = lt & 31, wid = lt >> 5;
+  const int64_t ntiles = (m + R - 1) / R;
+  for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int64_t r0 = t * R;
+    int d[2][8];   // the rows' offsets, INT_MAX where absent
+    bool fail = false;
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int64_t r = r0 + lt + q * H;
+      int b = 0, e = 0;
+      if (r < m) {
+        b = rowptr[r];
+        e = rowptr[r + 1];
+      }
+      fail |= e - b > 8;
+      int prev = -1;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const bool on = j < e - b;
+        const int c = on ? colind[b + j] : 0;
+        fail |= on && c <= prev;
+        prev = c;
+        d[q][j] = on ? c - (int)r : INT_MAX;
+      }
+    }
+    // uniform exit once any block has found the operator ineligible
+    if (__syncthreads_or(fail || (lt == 0 && *(volatile int *)bad))) {
+      if (fail) atomicExch(bad, 1);
+      return;
+    }
+    uint32_t mk[2] = {0u, 0u};
+    int last = INT_MIN, nb = 0;
+    for (int rd = 0;; ++rd) {
+      int v = INT_MAX;
+#pragma unroll
+      for (int q = 0; q < 2; ++q)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (d[q][j] > last && d[q][j] < v) v = d[q][j];
+      v = __reduce_min_sync(0xffffffffu, v);
+      if (lane == 0) red[rd & 1][wid] = v;   // double-buffered: the next round's writes cannot race this round's reads
+      __syncthreads();
+      int o = red[rd & 1][0];
+#pragma unroll
+      for (int w = 1; w < H / 32; ++w) o = min(o, red[rd & 1][w]);
+      if (o == INT_MAX) break;
+      if (rd == 8) {   // a ninth distinct offset
+        if (lt == 0) atomicExch(bad, 1);
+        return;
+      }
+#pragma unroll
+      for (int q = 0; q < 2; ++q)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          if (d[q][j] == o) mk[q] |= 1u << rd;
+      if (lt == 0) hdr[t].off[rd] = o;
+      last = o;
+      nb = rd + 1;
+    }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) mask[r0 + lt + q * H] = (uint8_t)mk[q];   // 0 for the rows past m of the last tile
+    if (lt < 8 && lt >= nb) hdr[t].off[lt] = 0;
+    if (lt == 0) {
+      hdr[t].nb = nb;
+      hdr[t].k0 = rowptr[r0];
+      hdr[t].k1 = rowptr[r0 + R < m ? r0 + R : m];
+      for (int p = 0; p < 5; ++p) hdr[t].pad[p] = 0;
+    }
+  }
+}
+
 template <typename T>
 __global__ void k_pack(const int *__restrict__ idx, const T *__restrict__ x, int64_t n, T *__restrict__ out) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x)
@@ -362,6 +444,28 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
         A->stream_lpr = 1 << l;
         break;
       }
+  }
+  // band description (csr.cuh): single GPU, and only worth a pass when no row has more than 8 nonzeros and the CSR
+  // stream runs with one lane per row
+  A->band_ok = false;
+  if (ctx->world == 1 && A->stream_lpr == 1 && A->max_row_nnz <= 8) {
+    const int64_t ntiles = (A->m_local + kBandTileRows - 1) / kBandTileRows;
+    B200_CUDA(cudaMalloc(&A->band_hdr, sizeof(b200_band_tile) * ntiles));
+    B200_CUDA(cudaMalloc(&A->band_mask, (size_t)kBandTileRows * ntiles));
+    int *d_bad = d_max + 7;
+    B200_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), ctx->stream));
+    k_band_build<<<grid_for(ctx, ntiles, 1), kBandBuildThreads, 0, ctx->stream>>>(A->rowptr, A->colind, A->m_local,
+                                                                                   A->band_hdr, A->band_mask, d_bad);
+    B200_LAUNCH_CHECK(ctx);
+    B200_CUDA(cudaMemcpyAsync(ctx->h_flags, d_bad, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    B200_CUDA(cudaStreamSynchronize(ctx->stream));
+    A->band_ok = ctx->h_flags[0] == 0;
+    if (!A->band_ok) {
+      cudaFree(A->band_hdr);
+      cudaFree(A->band_mask);
+      A->band_hdr = nullptr;
+      A->band_mask = nullptr;
+    }
   }
   B200_CUDA(cudaMemsetAsync(d_max, 0, sizeof(double) * 8, ctx->stream));
   // halo exchange lists
@@ -761,6 +865,8 @@ int b200_csr_destroy(b200_csr *A) {
   cudaFree(A->send_idx);
   cudaFree(A->send_buf);
   cudaFree(A->halo);
+  cudaFree(A->band_hdr);
+  cudaFree(A->band_mask);
   if (A->st_plan && A->st_plan_free) A->st_plan_free(A->st_plan);
   delete A;
   return B200_OK;
@@ -775,6 +881,23 @@ int b200_csr_info(const b200_csr *A, int64_t *m_local, int64_t *n_global, int64_
   if (dtype) *dtype = A->dtype;
   if (row_begin) *row_begin = A->row_begin;
   if (n_halo) *n_halo = A->n_halo;
+  return B200_OK;
+}
+
+int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes) {
+  B200_REQUIRE(A, "A is NULL");
+  const int64_t ntiles = (A->m_local + kBandTileRows - 1) / kBandTileRows;
+  int k;
+  int64_t bytes;
+  if (A->band_ok) {
+    k = 3;
+    bytes = ntiles * (int64_t)(sizeof(b200_band_tile) + kBandTileRows);
+  } else {
+    k = A->stream_lpr > 0 ? 2 : 1;
+    bytes = 4 * A->nnz + 4 * (A->m_local + 1);
+  }
+  if (kind) *kind = k;
+  if (structure_bytes) *structure_bytes = bytes;
   return B200_OK;
 }
 

@@ -17,9 +17,20 @@ namespace b200 {
 // inside the allocations (spmv_stream.cuh)
 constexpr int64_t kRowptrPad = 520;
 constexpr int64_t kNnzPad = 16;
+constexpr int kBandTileRows = 512;   // rows per tile of the band description (spmv_stream.cuh)
 }  // namespace b200
 using b200::kNnzPad;
 using b200::kRowptrPad;
+
+// Per-tile header of the band description.  Tile t covers rows [t*R, min(t*R+R, m)), R = kBandTileRows; its nonzeros are
+// vals[k0, k1) (= rowptr[r0], rowptr[r1]) in row order, and within a row in ascending offset order.
+struct alignas(16) b200_band_tile {
+  int off[8];   // the tile's distinct offsets col - row, ascending; entries >= nb are 0
+  int nb;       // number of offsets
+  int k0, k1;
+  int pad[5];
+};
+static_assert(sizeof(b200_band_tile) == 64, "band tile header is 64 bytes");
 
 struct b200_csr {
   b200_ctx *ctx = nullptr;
@@ -32,6 +43,12 @@ struct b200_csr {
   void *vals = nullptr;    // nnz
   int max_row_nnz = 0;
   double avg_row_nnz = 0.0;
+  // band description (single GPU, every 512-row tile has <= 8 distinct offsets col - row, columns strictly ascending
+  // in every row): the structure of the operator without colind/rowptr, consumed by the band-streamed SpMV
+  // (spmv_stream.cuh).  vals stay the CSR's own array.
+  bool band_ok = false;
+  struct b200_band_tile *band_hdr = nullptr;  // one 64-byte header per tile
+  uint8_t *band_mask = nullptr;               // one byte per row (padded to whole tiles): bit j = the row has offset j
   // halo exchange state (world > 1)
   std::vector<int64_t> send_count, send_offset, recv_count, recv_offset;  // per peer
   int64_t n_send = 0;

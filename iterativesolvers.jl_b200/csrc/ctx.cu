@@ -241,7 +241,7 @@ int b200_ctx_timer_stop(b200_ctx *c, float *ms) {
 int b200_ctx_set_option(b200_ctx *c, const char *name, int64_t value) {
   B200_REQUIRE(c && name, "NULL argument");
   if (strcmp(name, "spmv_kernel") == 0) {
-    B200_REQUIRE(value >= 0 && value <= 2, "spmv_kernel must be 0, 1 or 2");
+    B200_REQUIRE(value >= 0 && value <= 3, "spmv_kernel must be 0, 1, 2 or 3");
     c->opt_spmv_kernel = (int)value;
     return B200_OK;
   }

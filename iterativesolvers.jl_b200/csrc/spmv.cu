@@ -82,6 +82,27 @@ __global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
 }
 
 template <typename T>
+__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
+    k_spmv_band(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ x, int64_t nx, int64_t m,
+                T *__restrict__ y, const int *__restrict__ gate, int gate_mask) {
+  if (gate && (*gate & gate_mask)) return;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  StoreEpi<T> epi{y};
+  spmv_band_tiles<T>(ba, vals, x, nx, m, epi, reinterpret_cast<BandSmem<T> *>(smem_raw));
+}
+
+template <typename T>
+int launch_spmv_band(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate, int gate_mask) {
+  const int grid = stream_grid_size(ctx, A);
+  const size_t smem = sizeof(BandSmem<T>);
+  B200_SMEM_ATTR_ONCE(ctx, smem, k_spmv_band<T>);
+  k_spmv_band<T><<<grid, kStreamThreads, smem, ctx->stream>>>(make_band_args(A), (const T *)A->vals, (const T *)x,
+                                                              A->n_global, A->m_local, (T *)y, gate, gate_mask);
+  B200_LAUNCH_CHECK(ctx);
+  return B200_OK;
+}
+
+template <typename T>
 int launch_spmv_stream(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate, int gate_mask) {
   XView<T> xv = make_xview<T>(A, x);
   const int grid = stream_grid_size(ctx, A);
@@ -108,6 +129,7 @@ int launch_spmv_stream(b200_ctx *ctx, const b200_csr *A, const void *x, void *y,
 template <typename T>
 int launch_spmv(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate = nullptr, int gate_mask = 0) {
   if (A->m_local == 0) return B200_OK;
+  if (use_band(ctx, A, x)) return launch_spmv_band<T>(ctx, A, x, y, gate, gate_mask);
   if (use_stream(ctx, A)) return launch_spmv_stream<T>(ctx, A, x, y, gate, gate_mask);
   XView<T> xv = make_xview<T>(A, x);
   const int lpr = pick_lpr(A->avg_row_nnz);

@@ -28,6 +28,11 @@
 // the sub-warp kernel (spmv.cuh).  With LPR == 1 and fp64 the row sum is accumulated left to right
 // with separate multiply and add, i.e. bit-identical to SparseArrays' CSC scatter for a matrix given
 // with sorted columns.
+//
+// Operators with a band description (csr.cuh: <= 8 distinct offsets col - row per 512-row tile) take the second body
+// below, spmv_band_tiles: the same tiles and thread mapping, but the producer stages per-tile masks and contiguous
+// x bands instead of colind/rowptr, so a tile costs 8 B/nonzero + 1 B/row + 64 B of HBM structure and the consumers
+// no longer gather x from L1/L2 at all.
 #pragma once
 #include "spmv.cuh"
 
@@ -246,9 +251,253 @@ __device__ __forceinline__ void spmv_stream_tiles(const int *__restrict__ rowptr
 
 #endif  // __CUDACC__
 
+// ------------------------------------------------------------------------------------------------
+// Band-streamed form (operators with A->band_ok, csr.cuh): the structure of a tile of 512 rows is its <= 8 distinct
+// offsets d_j = col - row (the tile header, read by the producer one tile ahead) and one mask byte per row (bit j: the
+// row has offset d_j).  Every x operand of the tile then lies in the band x[r0+d_j, r0+d_j+rows), so the producer
+// bulk-copies, per stage: the tile's vals (evict-first, as above), its masks, and one x band per offset (default L2
+// policy: the bands are the L2 reuse the sweep order relies on).  Consumers touch only shared memory: a row's first
+// nonzero in the stage is the prefix popcount of the masks before it (one scan per group and tile), and the row sum is
+// taken over the set mask bits in ascending j = ascending column, left to right with unfused multiply and add --
+// bit-identical to the CSR stream.  Per SpMV this reads vals, 1 B/row of masks and 64 B/tile of headers instead of
+// 4 B/nonzero of colind and 4 B/row of rowptr.
+// ------------------------------------------------------------------------------------------------
+constexpr int kBandMax = 8;      // offsets per tile
+constexpr int kBandStages = 3;   // 3 x 66 KB (fp64) of the 227 KB of shared memory
+// the same tiles, rows per thread and CTA interleave as spmv_stream_tiles<T, 1>: every row result and every epilogue
+// partial sum (cg!'s dot(u, c)) is formed by the same thread in the same order, so the two forms are bit-identical
+static_assert(kBandTileRows == kStreamTileRows, "band tiles are the LPR == 1 stream tiles");
+
+template <typename T>
+struct alignas(128) BandStage {
+  T val[kStreamNnzCap + 8];
+  // band j holds x[bs_j, be_j): bs_j rounded down and be_j up to 16 bytes, so at most R + 2*(16/sizeof(T) - 1) entries
+  T xb[kBandMax][kStreamTileRows + 32 / sizeof(T)];
+  uint8_t mask[kStreamTileRows];
+};
+template <typename T>
+struct BandSmem {
+  BandStage<T> stage[kBandStages];
+  // written by the producer with ordinary stores before it arrives on full[s] (never a bulk-copy target):
+  // band[s][j] = {index in xb[j] of row 0's operand, entries copied, bs_j, 0}; kofs[s] = first nonzero - first copied
+  int4 band[kBandStages][kBandMax];
+  int kofs[kBandStages];
+  int fill[kBandStages];   // number of the last fill the producer started on each stage (-1: none yet)
+  int scan[kStreamGroups][2][kStreamGroupThreads / 32];
+  alignas(8) unsigned long long full[kBandStages];
+  alignas(8) unsigned long long empty[kBandStages];
+};
+
+struct BandArgs {
+  const b200_band_tile *hdr;
+  const uint8_t *mask;
+};
+inline BandArgs make_band_args(const b200_csr *A) { return BandArgs{A->band_hdr, A->band_mask}; }
+
+#ifdef __CUDACC__
+
+__device__ __forceinline__ int ld_acquire_shared(const int *p) {
+  int v;
+  asm volatile("ld.acquire.cta.shared::cta.b32 %0, [%1];" : "=r"(v) : "r"(smem_u32(p)) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_release_shared(int *p, int v) {
+  asm volatile("st.release.cta.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(p)), "r"(v) : "memory");
+}
+
+__device__ __forceinline__ void bulk_g2s_plain(void *dst_smem, const void *src_gmem, uint32_t bytes,
+                                               unsigned long long *bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+
+// Same contract as spmv_stream_tiles (LPR == 1): `x` (nx entries, 16-byte aligned) is the operand, m the rows.
+template <typename T, typename Epi>
+__device__ __forceinline__ void spmv_band_tiles(const BandArgs ba, const T *__restrict__ vals, const T *__restrict__ x,
+                                                int64_t nx, int64_t m, Epi &epi, BandSmem<T> *sm, bool rev = false) {
+  constexpr int R = kStreamTileRows;
+  constexpr int SLOTS = kStreamGroupThreads;
+  constexpr int AL = 16 / (int)sizeof(T);   // elements per 16 bytes
+  const int tid = threadIdx.x;
+  const int64_t ntiles = (m + R - 1) / R;
+  auto phys = [&](int64_t seq) -> int64_t { return rev ? ntiles - 1 - seq : seq; };
+  if (tid == 0) {
+    for (int s = 0; s < kBandStages; ++s) {
+      mbar_init(&sm->full[s], 1);
+      mbar_init(&sm->empty[s], kStreamGroupThreads / 32);
+      sm->fill[s] = -1;
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (tid >= kStreamConsumers) {
+    // ------------------------------------------------------------ producer warp
+    if (tid == kStreamConsumers) {
+      const uint64_t pol_stream = policy_evict_first();
+      const int64_t nxa = nx & ~(int64_t)(AL - 1);   // bands never copy past the last whole 16 bytes of x
+      int64_t t = blockIdx.x;
+      // the header of the next tile is fetched one iteration ahead (off the critical path)
+      int4 h0 = make_int4(0, 0, 0, 0), h1 = h0, h2 = h0;
+      if (t < ntiles) {
+        const int4 *p = reinterpret_cast<const int4 *>(ba.hdr + phys(t));
+        h0 = __ldg(p);
+        h1 = __ldg(p + 1);
+        h2 = __ldg(p + 2);
+      }
+      for (int it = 0; t < ntiles; ++it) {
+        const int s = it % kBandStages;
+        const uint32_t ph = (uint32_t)((it / kBandStages) & 1);
+        const int64_t r0 = phys(t) * R;
+        const int64_t rows = (r0 + R < m) ? R : m - r0;
+        const int64_t tn = t + gridDim.x;
+        int4 n0 = make_int4(0, 0, 0, 0), n1 = n0, n2 = n0;
+        if (tn < ntiles) {
+          const int4 *p = reinterpret_cast<const int4 *>(ba.hdr + phys(tn));
+          n0 = __ldg(p);
+          n1 = __ldg(p + 1);
+          n2 = __ldg(p + 2);
+        }
+        const int off[kBandMax] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+        const int nb = h2.x, k0 = h2.y, k1 = h2.z;
+        mbar_wait(&sm->empty[s], ph ^ 1u);
+        const int k0a = k0 & ~3;
+        const uint32_t b_val = (uint32_t)(((k1 - k0a) + 3) & ~3) * (uint32_t)sizeof(T);
+        uint32_t total = b_val + (uint32_t)R;
+        int64_t bsj[kBandMax];
+        uint32_t bb[kBandMax];
+#pragma unroll
+        for (int j = 0; j < kBandMax; ++j) {
+          int4 e = make_int4(0, 0, 0, 0);
+          bsj[j] = 0;
+          bb[j] = 0;
+          if (j < nb) {
+            // clamp the band to [0, nx); masks guarantee no row of the tile reads outside it
+            const int64_t lo = r0 + off[j] > 0 ? r0 + off[j] : 0;
+            const int64_t hi = r0 + off[j] + rows < nx ? r0 + off[j] + rows : nx;
+            const int64_t bs = lo & ~(int64_t)(AL - 1);
+            const int64_t be_up = (hi + AL - 1) & ~(int64_t)(AL - 1);
+            const int64_t be = be_up < nxa ? be_up : nxa;
+            const int64_t cnt = be > bs ? be - bs : 0;
+            e = make_int4((int)(r0 + off[j] - bs), (int)cnt, (int)bs, 0);
+            bsj[j] = bs;
+            bb[j] = (uint32_t)cnt * (uint32_t)sizeof(T);
+            total += bb[j];
+          }
+          sm->band[s][j] = e;
+        }
+        sm->kofs[s] = k0 - k0a;
+        st_release_shared(&sm->fill[s], it / kBandStages);   // see the consumers' wait
+        BandStage<T> *st = &sm->stage[s];
+        mbar_expect_tx(&sm->full[s], total);   // releases the ordinary stores above together with the arrival
+        bulk_g2s(st->mask, ba.mask + r0, (uint32_t)R, &sm->full[s], pol_stream);
+        bulk_g2s(st->val, vals + k0a, b_val, &sm->full[s], pol_stream);
+#pragma unroll
+        for (int j = 0; j < kBandMax; ++j)
+          if (bb[j]) bulk_g2s_plain(st->xb[j], x + bsj[j], bb[j], &sm->full[s]);
+        t = tn;
+        h0 = n0;
+        h1 = n1;
+        h2 = n2;
+      }
+    }
+  } else {
+    // ------------------------------------------------------------ consumers: group g takes tiles k = g, g+2, ...
+    const int grp = tid / kStreamGroupThreads;
+    const int slot = tid % kStreamGroupThreads;
+    const int lane = tid & 31, wig = slot >> 5;   // warp in group
+    // the epilogue's own per-row operands (e.g. cg!'s u[row]) are loaded one tile of the group ahead, so that their
+    // latency overlaps the current tile instead of stalling its epilogue; the kernel does not write what they read
+    auto pre_of = [&](int64_t kk, T (&p)[2]) {
+      const int64_t tt = (int64_t)blockIdx.x + kk * gridDim.x;
+      const int64_t row = tt < ntiles ? phys(tt) * R + slot : m;
+      p[0] = row < m ? epi.pre(row) : (T)0;
+      p[1] = row + SLOTS < m ? epi.pre(row + SLOTS) : (T)0;
+    };
+    T pre_next[2];
+    pre_of(grp, pre_next);
+    for (int64_t k = grp;; k += kStreamGroups) {
+      const int64_t t = (int64_t)blockIdx.x + k * gridDim.x;
+      if (t >= ntiles) break;
+      const int s = (int)(k % kBandStages);
+      const uint32_t ph = (uint32_t)((k / kBandStages) & 1);
+      const int64_t r0 = phys(t) * R;
+      const bool valid0 = r0 + slot < m, valid1 = r0 + slot + SLOTS < m;
+      const T pre[2] = {pre_next[0], pre_next[1]};
+      pre_of(k + kStreamGroups, pre_next);
+      // With 3 stages and 2 groups, consecutive fills of a stage belong to DIFFERENT groups (tile k - 3 is the other
+      // group's), so this group can reach its wait for fill n = k/3 of stage s while fill n - 1 is still landing.  The
+      // parity of fill n is that of fill n - 2, long complete, so a parity wait alone would return at once: the group
+      // would read a stage that is still being written and arrive on the wrong phase of empty[s], desynchronising the
+      // ring until it hangs.  The producer therefore publishes the number of the fill it has started on each stage;
+      // once that is n, fill n - 1 has been consumed (the producer waited for it) and fill n + 1 cannot start before
+      // this group releases the stage, so the parity wait refers to fill n alone.
+      const int fill_no = (int)(k / kBandStages);
+      while (ld_acquire_shared(&sm->fill[s]) != fill_no) __nanosleep(32);
+      mbar_wait(&sm->full[s], ph);
+      const BandStage<T> *st = &sm->stage[s];
+      const uint32_t mk0 = st->mask[slot], mk1 = st->mask[slot + SLOTS];   // 0 past the last row
+      // row starts: exclusive prefix of the popcounts over the group, both rows' counts packed in one int
+      const int own = __popc(mk0) | (__popc(mk1) << 16);
+      int inc = own;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += v;
+      }
+      int *scan = sm->scan[grp][(k / kStreamGroups) & 1];
+      if (lane == 31) scan[wig] = inc;
+      asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(kStreamGroupThreads) : "memory");
+      int before = 0, all = 0;
+#pragma unroll
+      for (int w = 0; w < kStreamGroupThreads / 32; ++w) {
+        const int v = scan[w];
+        if (w < wig) before += v;
+        all += v;
+      }
+      const int excl = before + inc - own;
+      const int kofs = sm->kofs[s];
+      int kk0 = kofs + (excl & 0xffff);
+      int kk1 = kofs + (all & 0xffff) + (excl >> 16);
+      T acc[2] = {(T)0, (T)0};
+      // left-to-right, unfused multiply-add in ascending column order (see the comment above)
+#pragma unroll
+      for (int j = 0; j < kBandMax; ++j) {
+        const int4 bj = sm->band[s][j];
+        if ((mk0 >> j) & 1u) {
+          const int p = slot + bj.x;
+          const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
+          if constexpr (sizeof(T) == 8) acc[0] = __dadd_rn(acc[0], __dmul_rn(st->val[kk0], xj));
+          else acc[0] = __fadd_rn(acc[0], __fmul_rn(st->val[kk0], xj));
+          ++kk0;
+        }
+        if ((mk1 >> j) & 1u) {
+          const int p = slot + SLOTS + bj.x;
+          const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
+          if constexpr (sizeof(T) == 8) acc[1] = __dadd_rn(acc[1], __dmul_rn(st->val[kk1], xj));
+          else acc[1] = __fadd_rn(acc[1], __fmul_rn(st->val[kk1], xj));
+          ++kk1;
+        }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&sm->empty[s]);   // the stage is no longer read; the epilogue touches global memory only
+      if (valid0) epi(r0 + slot, acc[0], pre[0]);
+      if (valid1) epi(r0 + slot + SLOTS, acc[1], pre[1]);
+    }
+  }
+}
+
+#endif  // __CUDACC__
+
 // true if the TMA-streamed kernel serves this operator (tiles fit, not overridden by the option)
 inline bool use_stream(const b200_ctx *ctx, const b200_csr *A) {
   return A->stream_lpr > 0 && ctx->opt_spmv_kernel != 1;
+}
+// true if the band-streamed form serves y = A x: the operator has a band description, the option is auto (0) or
+// band (3), and x is 16-byte aligned (bulk copies; user vectors may be offset views)
+inline bool use_band(const b200_ctx *ctx, const b200_csr *A, const void *x) {
+  return A->band_ok && (ctx->opt_spmv_kernel == 0 || ctx->opt_spmv_kernel == 3) && ((uintptr_t)x & 15u) == 0;
 }
 inline int stream_grid_size(const b200_ctx *ctx, const b200_csr *A) {
   const int R = kStreamTileRows / A->stream_lpr;
