@@ -25,7 +25,7 @@
 #include <cooperative_groups.h>
 
 #include "blas1.cuh"
-#include "spmv_stream.cuh"
+#include "spmv_launch.cuh"
 #include "linop.cuh"
 
 using namespace b200;
@@ -223,85 +223,42 @@ __global__ void __launch_bounds__(kThreads) k_cg_flush_x(const T *__restrict__ u
 }
 
 
-// K2 (sub-warp-per-row fallback): c = A*u ; sum u.*c
-template <typename T, int LPR>
-__global__ void __launch_bounds__(kThreads) k_cg_spmv_dot(const int *__restrict__ rowptr,
-                                                          const int *__restrict__ colind,
-                                                          const T *__restrict__ vals, XView<T> xv, int64_t m,
-                                                          T *__restrict__ c, CgScal *s, double *partials,
-                                                          unsigned int *ticket, Comm cm) {
-  pdl_wait();
-  if (s->done) return;
-  __shared__ double smem[kThreads / 32];
-  wait_halo(cm);
-  constexpr int ROWS = kThreads / LPR;
-  const int sub = threadIdx.x % LPR;
-  const int rib = threadIdx.x / LPR;
-  double acc = 0.0;
-  for (int64_t base = (int64_t)blockIdx.x * ROWS; base < m; base += (int64_t)gridDim.x * ROWS) {
-    const int64_t row = base + rib;
-    const bool valid = row < m;
-    const T ci = row_dot<T, LPR>(rowptr, colind, vals, xv, valid ? row : (m - 1), sub);
-    if (valid && sub == 0) {
-      c[row] = ci;
-      acc += (double)xv.x[row] * (double)ci;
-    }
-  }
-  pdl_launch_dependents();
-  acc = block_sum<kThreads>(acc, smem);
-  double total;
-  if (grid_reduce_finish<kThreads>(acc, partials, ticket, smem, &total) && threadIdx.x < 32)
-    cg_finish(FIN_DOT, s, total, nullptr, cm);
-}
-
-// K2, TMA-streamed form (spmv_stream.cuh): same result contract as k_cg_spmv_dot
+// K2: c = A*u fused with dot(u, c), the epilogue of the SpMV kernels (spmv_launch.cuh)
 template <typename T>
 struct CgDotEpi {
   T *__restrict__ c;
   const T *__restrict__ u;
+  CgScal *s;
+  double *partials;
+  unsigned int *ticket;
+  Comm cm;
   double acc;
+  // wait_halo and cg_finish get a copy of cm: they index cm.pv.hdr by rank, which would otherwise keep the whole
+  // epilogue, acc included, in local memory
+  __device__ __forceinline__ bool begin() {
+    pdl_wait();
+    if (s->done) return false;
+    const Comm c = cm;
+    wait_halo(c);
+    return true;
+  }
   __device__ __forceinline__ T pre(int64_t row) const { return u[row]; }
   __device__ __forceinline__ void operator()(int64_t row, T v, T ur) {
     c[row] = v;
     acc += (double)ur * (double)v;
   }
+  template <int THREADS>
+  __device__ __forceinline__ void end(double *red) {
+    pdl_launch_dependents();
+    const double a = block_sum<THREADS>(acc, red);
+    double total;
+    if (grid_reduce_finish<THREADS>(a, partials, ticket, red, &total) && threadIdx.x < 32) {
+      const Comm c = cm;
+      cg_finish(FIN_DOT, s, total, nullptr, c);
+    }
+  }
+  __device__ __forceinline__ bool rev() const { return cm.rev != 0; }
 };
-template <typename T, int LPR>
-__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
-    k_cg_spmv_dot_stream(const int *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
-                         XView<T> xv, int64_t m, T *__restrict__ c, CgScal *s, double *partials,
-                         unsigned int *ticket, Comm cm) {
-  pdl_wait();
-  if (s->done) return;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ double red[kStreamThreads / 32];
-  wait_halo(cm);
-  CgDotEpi<T> epi{c, xv.x, 0.0};
-  spmv_stream_tiles<T, LPR>(rowptr, colind, vals, xv, m, epi, reinterpret_cast<StreamSmem<T> *>(smem_raw), cm.rev != 0);
-  pdl_launch_dependents();
-  const double acc = block_sum<kStreamThreads>(epi.acc, red);
-  double total;
-  if (grid_reduce_finish<kStreamThreads>(acc, partials, ticket, red, &total) && threadIdx.x < 32)
-    cg_finish(FIN_DOT, s, total, nullptr, cm);
-}
-
-// K2, band-streamed form (single GPU, operators with a band description): same result contract
-template <typename T>
-__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
-    k_cg_spmv_dot_band(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ u, int64_t m,
-                       T *__restrict__ c, CgScal *s, double *partials, unsigned int *ticket, Comm cm) {
-  pdl_wait();
-  if (s->done) return;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ double red[kStreamThreads / 32];
-  CgDotEpi<T> epi{c, u, 0.0};
-  spmv_band_tiles<T>(ba, vals, u, m, m, epi, reinterpret_cast<BandSmem<T> *>(smem_raw), cm.rev != 0);
-  pdl_launch_dependents();
-  const double acc = block_sum<kStreamThreads>(epi.acc, red);
-  double total;
-  if (grid_reduce_finish<kStreamThreads>(acc, partials, ticket, red, &total) && threadIdx.x < 32)
-    cg_finish(FIN_DOT, s, total, nullptr, cm);
-}
 
 // K3: r -= alpha*c ; ||r||^2   (x += alpha*u is applied by the next K1 / k_cg_flush_x)
 template <typename T>
@@ -504,6 +461,11 @@ __global__ void __launch_bounds__(kThreads) k_cg_persistent(const int *__restric
 }
 
 template <typename T>
+const void *cg_persistent_kernel(int lpr) {
+  return with_lpr<2>(lpr, [](auto l) { return (const void *)k_cg_persistent<T, decltype(l)::value>; });
+}
+
+template <typename T>
 struct CgEngine {
   b200_ctx *ctx;
   const b200_csr *A;
@@ -514,7 +476,7 @@ struct CgEngine {
   CgScal *s;
   double *hist;
   int mode;      // COMM_*
-  int lpr, grid_vec, grid_spmv;
+  int lpr, grid_vec;
   int sweep = 0;   // direction of the next hot kernel (toggled per launch when ctx->opt_snake)
   bool fold_halo = false;   // peer path, Identity: r's boundary is pushed after K3 and K1 forms u's halo locally
   bool fold_push = false;   // ... and K3 itself stores the boundary rows to the neighbours (contiguous send ranges)
@@ -564,52 +526,13 @@ struct CgEngine {
     } else {
       B200_TRY(halo_exchange(ctx, A, u));
     }
-    XView<T> xv = make_xview<T>(A, u, peer && !fold_halo);
     const Comm cm = comm(!fold_halo, next_sweep());
-    if (use_band(ctx, A, u)) {
-      const int grid = stream_grid_size(ctx, A);
-      const size_t smem = sizeof(BandSmem<T>);
+    {
       ProfScope prof(ctx, 0);
-      B200_SMEM_ATTR_ONCE(ctx, smem, k_cg_spmv_dot_band<T>);
-      B200_CUDA(launch_chained(ctx->opt_pdl != 0, k_cg_spmv_dot_band<T>, dim3(grid), dim3(kStreamThreads), smem,
-                               ctx->stream, make_band_args(A), (const T *)A->vals, (const T *)u, n, c, s,
-                               ctx->red.partials, ctx->red.ticket, cm));
-    } else if (use_stream(ctx, A)) {
-      const int grid = stream_grid_size(ctx, A);
-      const size_t smem = sizeof(StreamSmem<T>);
-      ProfScope prof(ctx, 0);
-#define LAUNCH(L)                                                                                                    \
-  do {                                                                                                               \
-    B200_SMEM_ATTR_ONCE(ctx, smem, k_cg_spmv_dot_stream<T, L>);                                                      \
-    B200_CUDA(launch_chained(ctx->opt_pdl != 0, k_cg_spmv_dot_stream<T, L>, dim3(grid), dim3(kStreamThreads), smem,    \
-                             ctx->stream, A->rowptr, A->colind, (const T *)A->vals, xv, n, c, s, ctx->red.partials,  \
-                             ctx->red.ticket, cm));                                                                  \
-  } while (0)
-      switch (A->stream_lpr) {
-        case 1: LAUNCH(1); break;
-        case 2: LAUNCH(2); break;
-        case 4: LAUNCH(4); break;
-        case 8: LAUNCH(8); break;
-        case 16: LAUNCH(16); break;
-        default: LAUNCH(32); break;
-      }
-#undef LAUNCH
-    } else {
-      ProfScope prof(ctx, 0);
-#define LAUNCH(L)                                                                                               \
-  B200_CUDA(launch_chained(ctx->opt_pdl != 0, k_cg_spmv_dot<T, L>, dim3(grid_spmv), dim3(kThreads), 0, ctx->stream, \
-                           A->rowptr, A->colind, (const T *)A->vals, xv, n, c, s, ctx->red.partials,             \
-                           ctx->red.ticket, cm))
-      switch (lpr) {
-        case 2: LAUNCH(2); break;
-        case 4: LAUNCH(4); break;
-        case 8: LAUNCH(8); break;
-        case 16: LAUNCH(16); break;
-        default: LAUNCH(32); break;
-      }
-#undef LAUNCH
+      B200_TRY(launch_spmv_fused<T>(ctx, A, u, peer && !fold_halo,
+                                    CgDotEpi<T>{c, u, s, ctx->red.partials, ctx->red.ticket, cm, 0.0},
+                                    ctx->opt_pdl != 0));
     }
-    B200_LAUNCH_CHECK(ctx);
     return after_reduce(FIN_DOT);
   }
 
@@ -680,16 +603,9 @@ struct CgEngine {
     long long kk = k;
     void *args[] = {(void *)&rp, (void *)&ci, (void *)&va, (void *)&jc, (void *)&x_, (void *)&r_, (void *)&u_, (void *)&c_,
                     (void *)&n_, (void *)&s_, (void *)&h_, (void *)&pt, (void *)&kk};
-    const void *kern = nullptr;
-    switch (lpr) {
-      case 2: kern = (const void *)k_cg_persistent<T, 2>; break;
-      case 4: kern = (const void *)k_cg_persistent<T, 4>; break;
-      case 8: kern = (const void *)k_cg_persistent<T, 8>; break;
-      case 16: kern = (const void *)k_cg_persistent<T, 16>; break;
-      default: kern = (const void *)k_cg_persistent<T, 32>; break;
-    }
     ProfScope prof(ctx, 0);
-    B200_CUDA(cudaLaunchCooperativeKernel(kern, dim3(grid_persist), dim3(kThreads), args, 0, ctx->stream));
+    B200_CUDA(cudaLaunchCooperativeKernel(cg_persistent_kernel<T>(lpr), dim3(grid_persist), dim3(kThreads), args, 0,
+                                          ctx->stream));
     ctx->launches++;
     return B200_OK;
   }
@@ -728,21 +644,13 @@ int cg_setup(CgEngine<T> &e, b200_ctx *ctx, const b200_csr *A, T *x, const T *b,
   e.mode = ctx->world == 1 ? COMM_SINGLE : (use_peer(ctx, A) ? COMM_PEER : COMM_NCCL);
   e.lpr = pick_lpr(A->avg_row_nnz);
   e.grid_vec = stream_grid(ctx, n, kThreads * 2, 8);
-  e.grid_spmv = stream_grid(ctx, n, kThreads / e.lpr, 8);
   e.fold_halo = e.mode == COMM_PEER && !e.jac && A->halo && A->halo_peer && A->n_halo > 0;
   if (e.fold_halo) B200_CUDA(cudaMemsetAsync(A->halo, 0, sizeof(T) * (size_t)A->n_halo, st));   // u_0 = 0
   e.persistent = false;
   if (ctx->world == 1 && ctx->opt_cg_persistent != 0 && n > 0 && n <= kPersistMaxRows) {
     int per_sm = 0;
-    const void *kern = nullptr;
-    switch (e.lpr) {
-      case 2: kern = (const void *)k_cg_persistent<T, 2>; break;
-      case 4: kern = (const void *)k_cg_persistent<T, 4>; break;
-      case 8: kern = (const void *)k_cg_persistent<T, 8>; break;
-      case 16: kern = (const void *)k_cg_persistent<T, 16>; break;
-      default: kern = (const void *)k_cg_persistent<T, 32>; break;
-    }
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, 0) == cudaSuccess && per_sm >= 1) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cg_persistent_kernel<T>(e.lpr), kThreads, 0) == cudaSuccess &&
+        per_sm >= 1) {
       const int64_t want = (n + (kThreads / e.lpr) - 1) / (kThreads / e.lpr);          // one SpMV row group per block
       const int64_t cap = std::min<int64_t>((int64_t)ctx->sm_count * std::min(per_sm, 2), kMaxPartials);
       e.grid_persist = (int)std::max<int64_t>(1, std::min<int64_t>(want, cap));

@@ -8,7 +8,7 @@
 // The vector "rotation" of :147-148 is a pointer swap done by the host (it is unconditional).
 // Algorithmic bytes per iteration: nnz*(V+4) + (n+1)*4 + 14*n*V.
 #include "blas1.cuh"
-#include "spmv_stream.cuh"
+#include "spmv_launch.cuh"
 
 using namespace b200;
 
@@ -134,83 +134,40 @@ __global__ void __launch_bounds__(kThreads) k_mr_scale(T *__restrict__ v, int64_
     v[i] = v[i] * inv;
 }
 
-// Ka
-template <typename T, int LPR>
-__global__ void __launch_bounds__(kThreads) k_mr_spmv(const int *__restrict__ rowptr, const int *__restrict__ colind,
-                                                      const T *__restrict__ vals, XView<T> xv,
-                                                      const T *__restrict__ v_prev, T *__restrict__ v_next,
-                                                      int64_t n, MrScal *m, double *partials, unsigned int *ticket,
-                                                      int single) {
-  if (m->done) return;
-  __shared__ double smem[kThreads / 32];
-  constexpr int ROWS = kThreads / LPR;
-  const int sub = threadIdx.x % LPR, rib = threadIdx.x / LPR;
-  const bool use_prev = m->iteration > 1;
-  const T h2 = (T)m->H[1];
-  double acc = 0.0;
-  for (int64_t base = (int64_t)blockIdx.x * ROWS; base < n; base += (int64_t)gridDim.x * ROWS) {
-    const int64_t row = base + rib;
-    const bool valid = row < n;
-    T t = row_dot<T, LPR>(rowptr, colind, vals, xv, valid ? row : (n - 1), sub);
-    if (valid && sub == 0) {
-      if (use_prev) t = t - h2 * v_prev[row];                                   // axpy!(-H[2], v_prev, v_next) :106
-      v_next[row] = t;
-      acc += (double)xv.x[row] * (double)t;                                     // dot(v_curr, v_next) :109
-    }
-  }
-  acc = block_sum<kThreads>(acc, smem);
-  double total;
-  if (grid_reduce_finish<kThreads>(acc, partials, ticket, smem, &total) && threadIdx.x == 0)
-    mr_finish(MR_PROJ, m, total, nullptr, single);
-}
-
-// Ka, TMA-streamed form (spmv_stream.cuh)
+// Ka: v_next = A v_curr - H[2] v_prev fused with dot(v_curr, v_next), the epilogue of the SpMV kernels (spmv_launch.cuh)
 template <typename T>
 struct MrEpi {
   T *__restrict__ v_next;
   const T *__restrict__ v_prev;
   const T *__restrict__ v_curr;
-  T h2;
+  MrScal *m;
+  double *partials;
+  unsigned int *ticket;
+  int single;
+  T h2;            // set by begin()
   bool use_prev;
   double acc;
+  __device__ __forceinline__ bool begin() {
+    if (m->done) return false;
+    h2 = (T)m->H[1];
+    use_prev = m->iteration > 1;
+    return true;
+  }
   __device__ __forceinline__ T pre(int64_t row) const { return use_prev ? v_prev[row] : (T)0; }
   __device__ __forceinline__ void operator()(int64_t row, T t, T vp) {
-    if (use_prev) t = t - h2 * vp;
+    if (use_prev) t = t - h2 * vp;                                              // axpy!(-H[2], v_prev, v_next) :106
     v_next[row] = t;
-    acc += (double)v_curr[row] * (double)t;
+    acc += (double)v_curr[row] * (double)t;                                     // dot(v_curr, v_next) :109
   }
+  template <int THREADS>
+  __device__ __forceinline__ void end(double *red) {
+    const double a = block_sum<THREADS>(acc, red);
+    double total;
+    if (grid_reduce_finish<THREADS>(a, partials, ticket, red, &total) && threadIdx.x == 0)
+      mr_finish(MR_PROJ, m, total, nullptr, single);
+  }
+  __device__ static constexpr bool rev() { return false; }
 };
-template <typename T, int LPR>
-__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
-    k_mr_spmv_stream(const int *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
-                     XView<T> xv, const T *__restrict__ v_prev, T *__restrict__ v_next, int64_t n, MrScal *m,
-                     double *partials, unsigned int *ticket, int single) {
-  if (m->done) return;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ double red[kStreamThreads / 32];
-  MrEpi<T> epi{v_next, v_prev, xv.x, (T)m->H[1], m->iteration > 1, 0.0};
-  spmv_stream_tiles<T, LPR>(rowptr, colind, vals, xv, n, epi, reinterpret_cast<StreamSmem<T> *>(smem_raw));
-  const double acc = block_sum<kStreamThreads>(epi.acc, red);
-  double total;
-  if (grid_reduce_finish<kStreamThreads>(acc, partials, ticket, red, &total) && threadIdx.x == 0)
-    mr_finish(MR_PROJ, m, total, nullptr, single);
-}
-
-// Ka, band-streamed form (single GPU, operators with a band description)
-template <typename T>
-__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
-    k_mr_spmv_band(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ v_curr, const T *__restrict__ v_prev,
-                   T *__restrict__ v_next, int64_t n, MrScal *m, double *partials, unsigned int *ticket, int single) {
-  if (m->done) return;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ double red[kStreamThreads / 32];
-  MrEpi<T> epi{v_next, v_prev, v_curr, (T)m->H[1], m->iteration > 1, 0.0};
-  spmv_band_tiles<T>(ba, vals, v_curr, n, n, epi, reinterpret_cast<BandSmem<T> *>(smem_raw));
-  const double acc = block_sum<kStreamThreads>(epi.acc, red);
-  double total;
-  if (grid_reduce_finish<kStreamThreads>(acc, partials, ticket, red, &total) && threadIdx.x == 0)
-    mr_finish(MR_PROJ, m, total, nullptr, single);
-}
 
 // Kb
 template <typename T>
@@ -292,8 +249,6 @@ int minres_impl(b200_ctx *ctx, const b200_csr *A, T *x, const T *b, const b200_m
   h.skew = o->skew_hermitian;
   B200_CUDA(cudaMemcpyAsync(m, &h, sizeof(h), cudaMemcpyHostToDevice, st));
   const int gv = stream_grid(ctx, n, kThreads * 2, 8);
-  const int lpr = pick_lpr(A->avg_row_nnz);
-  const int gs = stream_grid(ctx, n, kThreads / lpr, 8);
 
   auto after = [&](int kind) -> int {
     if (single) return B200_OK;
@@ -328,49 +283,12 @@ int minres_impl(b200_ctx *ctx, const b200_csr *A, T *x, const T *b, const b200_m
     const int64_t batch = std::min<int64_t>(check_every, maxiter - enqueued);
     for (int64_t it = 0; it < batch; ++it) {
       B200_TRY(halo_exchange(ctx, A, v_curr));
-      XView<T> xv = make_xview<T>(A, v_curr);
-      if (use_band(ctx, A, v_curr)) {
-        const int grid = stream_grid_size(ctx, A);
-        const size_t smem = sizeof(BandSmem<T>);
+      {
         ProfScope prof(ctx, 0);
-        B200_SMEM_ATTR_ONCE(ctx, smem, k_mr_spmv_band<T>);
-        k_mr_spmv_band<T><<<grid, kStreamThreads, smem, st>>>(make_band_args(A), (const T *)A->vals, v_curr, v_prev,
-                                                              v_next, n, m, ctx->red.partials, ctx->red.ticket, single);
-      } else if (use_stream(ctx, A)) {
-        const int grid = stream_grid_size(ctx, A);
-        const size_t smem = sizeof(StreamSmem<T>);
-        ProfScope prof(ctx, 0);
-#define LAUNCH(L)                                                                                                  \
-  do {                                                                                                             \
-    B200_SMEM_ATTR_ONCE(ctx, smem, k_mr_spmv_stream<T, L>);                                                        \
-    k_mr_spmv_stream<T, L><<<grid, kStreamThreads, smem, st>>>(A->rowptr, A->colind, (const T *)A->vals, xv,       \
-                                                                v_prev, v_next, n, m, ctx->red.partials,           \
-                                                                ctx->red.ticket, single);                          \
-  } while (0)
-        switch (A->stream_lpr) {
-          case 1: LAUNCH(1); break;
-          case 2: LAUNCH(2); break;
-          case 4: LAUNCH(4); break;
-          case 8: LAUNCH(8); break;
-          case 16: LAUNCH(16); break;
-          default: LAUNCH(32); break;
-        }
-#undef LAUNCH
-      } else {
-        ProfScope prof(ctx, 0);
-#define LAUNCH(L)                                                                                            \
-  k_mr_spmv<T, L><<<gs, kThreads, 0, st>>>(A->rowptr, A->colind, (const T *)A->vals, xv, v_prev, v_next, n, m, \
-                                           ctx->red.partials, ctx->red.ticket, single)
-        switch (lpr) {
-          case 2: LAUNCH(2); break;
-          case 4: LAUNCH(4); break;
-          case 8: LAUNCH(8); break;
-          case 16: LAUNCH(16); break;
-          default: LAUNCH(32); break;
-        }
-#undef LAUNCH
+        B200_TRY(launch_spmv_fused<T>(ctx, A, v_curr, false,
+                                      MrEpi<T>{v_next, v_prev, v_curr, m, ctx->red.partials, ctx->red.ticket, single},
+                                      false));
       }
-      B200_LAUNCH_CHECK(ctx);
       B200_TRY(after(MR_PROJ));
       {
         ProfScope prof(ctx, 1);

@@ -1,5 +1,5 @@
 // spmv.cu -- mul!(y, A, x) and mul!(Y, A, X) (block SpMM) on the device CSR.
-#include "spmv_stream.cuh"
+#include "spmv_launch.cuh"
 
 using namespace b200;
 
@@ -7,23 +7,20 @@ namespace {
 
 constexpr int kThreads = 256;
 
-// y = A x.  Sub-warp (LPR lanes) per row; blocks stride the rows in interleaved chunks so that all
-// resident blocks work on neighbouring rows (keeps the x planes of a stencil matrix in L2).
-template <typename T, int LPR>
-__global__ void __launch_bounds__(kThreads) k_spmv(const int *__restrict__ rowptr, const int *__restrict__ colind,
-                                                   const T *__restrict__ vals, XView<T> xv, int64_t m,
-                                                   T *__restrict__ y, const int *__restrict__ gate, int gate_mask) {
-  if (gate && (*gate & gate_mask)) return;   // speculatively enqueued launch whose solver has already stopped
-  constexpr int ROWS = kThreads / LPR;
-  const int sub = threadIdx.x % LPR;
-  const int rib = threadIdx.x / LPR;
-  for (int64_t base = (int64_t)blockIdx.x * ROWS; base < m; base += (int64_t)gridDim.x * ROWS) {
-    const int64_t row = base + rib;
-    const bool valid = row < m;
-    T s = row_dot<T, LPR>(rowptr, colind, vals, xv, valid ? row : (m - 1), sub);
-    if (valid && sub == 0) y[row] = s;
-  }
-}
+// y = A x (spmv_launch.cuh)
+template <typename T>
+struct StoreEpi {
+  T *__restrict__ y;
+  const int *__restrict__ gate;
+  int gate_mask;
+  // a speculatively enqueued launch whose solver has already stopped does nothing
+  __device__ __forceinline__ bool begin() const { return !(gate && (__ldg(gate) & gate_mask)); }
+  __device__ __forceinline__ T pre(int64_t) const { return (T)0; }
+  __device__ __forceinline__ void operator()(int64_t row, T v, T) { y[row] = v; }
+  template <int THREADS>
+  __device__ __forceinline__ void end(double *) const {}
+  __device__ static constexpr bool rev() { return false; }
+};
 
 // Y = A X for a column-major block of BS vectors: each sub-warp handles one row and keeps BS
 // accumulators, so A is streamed ONCE for the whole block (the CPU reference re-streams it per column).
@@ -64,90 +61,10 @@ __global__ void __launch_bounds__(kThreads) k_spmm(const int *__restrict__ rowpt
   }
 }
 
-// TMA-streamed y = A x (spmv_stream.cuh)
-template <typename T>
-struct StoreEpi {
-  T *__restrict__ y;
-  __device__ __forceinline__ T pre(int64_t) const { return (T)0; }
-  __device__ __forceinline__ void operator()(int64_t row, T v, T) { y[row] = v; }
-};
-template <typename T, int LPR>
-__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
-    k_spmv_stream(const int *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
-                  XView<T> xv, int64_t m, T *__restrict__ y, const int *__restrict__ gate, int gate_mask) {
-  if (gate && (*gate & gate_mask)) return;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  StoreEpi<T> epi{y};
-  spmv_stream_tiles<T, LPR>(rowptr, colind, vals, xv, m, epi, reinterpret_cast<StreamSmem<T> *>(smem_raw));
-}
-
-template <typename T>
-__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
-    k_spmv_band(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ x, int64_t nx, int64_t m,
-                T *__restrict__ y, const int *__restrict__ gate, int gate_mask) {
-  if (gate && (*gate & gate_mask)) return;
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  StoreEpi<T> epi{y};
-  spmv_band_tiles<T>(ba, vals, x, nx, m, epi, reinterpret_cast<BandSmem<T> *>(smem_raw));
-}
-
-template <typename T>
-int launch_spmv_band(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate, int gate_mask) {
-  const int grid = stream_grid_size(ctx, A);
-  const size_t smem = sizeof(BandSmem<T>);
-  B200_SMEM_ATTR_ONCE(ctx, smem, k_spmv_band<T>);
-  k_spmv_band<T><<<grid, kStreamThreads, smem, ctx->stream>>>(make_band_args(A), (const T *)A->vals, (const T *)x,
-                                                              A->n_global, A->m_local, (T *)y, gate, gate_mask);
-  B200_LAUNCH_CHECK(ctx);
-  return B200_OK;
-}
-
-template <typename T>
-int launch_spmv_stream(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate, int gate_mask) {
-  XView<T> xv = make_xview<T>(A, x);
-  const int grid = stream_grid_size(ctx, A);
-  const size_t smem = sizeof(StreamSmem<T>);
-#define LAUNCH(L)                                                                                                 \
-  do {                                                                                                            \
-    B200_SMEM_ATTR_ONCE(ctx, smem, k_spmv_stream<T, L>);                                                          \
-    k_spmv_stream<T, L><<<grid, kStreamThreads, smem, ctx->stream>>>(A->rowptr, A->colind, (const T *)A->vals,   \
-                                                                     xv, A->m_local, (T *)y, gate, gate_mask);  \
-  } while (0)
-  switch (A->stream_lpr) {
-    case 1: LAUNCH(1); break;
-    case 2: LAUNCH(2); break;
-    case 4: LAUNCH(4); break;
-    case 8: LAUNCH(8); break;
-    case 16: LAUNCH(16); break;
-    default: LAUNCH(32); break;
-  }
-#undef LAUNCH
-  B200_LAUNCH_CHECK(ctx);
-  return B200_OK;
-}
-
 template <typename T>
 int launch_spmv(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate = nullptr, int gate_mask = 0) {
   if (A->m_local == 0) return B200_OK;
-  if (use_band(ctx, A, x)) return launch_spmv_band<T>(ctx, A, x, y, gate, gate_mask);
-  if (use_stream(ctx, A)) return launch_spmv_stream<T>(ctx, A, x, y, gate, gate_mask);
-  XView<T> xv = make_xview<T>(A, x);
-  const int lpr = pick_lpr(A->avg_row_nnz);
-  const int rows = kThreads / lpr;
-  const int grid = stream_grid(ctx, A->m_local, rows, 8);
-#define LAUNCH(L)                                                                                             \
-  k_spmv<T, L><<<grid, kThreads, 0, ctx->stream>>>(A->rowptr, A->colind, (const T *)A->vals, xv, A->m_local, \
-                                                   (T *)y, gate, gate_mask)
-  switch (lpr) {
-    case 2: LAUNCH(2); break;
-    case 4: LAUNCH(4); break;
-    case 8: LAUNCH(8); break;
-    case 16: LAUNCH(16); break;
-    default: LAUNCH(32); break;
-  }
-#undef LAUNCH
-  B200_LAUNCH_CHECK(ctx);
-  return B200_OK;
+  return launch_spmv_fused<T>(ctx, A, x, false, StoreEpi<T>{(T *)y, gate, gate_mask}, false);
 }
 
 template <typename T, int BS>
@@ -158,17 +75,10 @@ int launch_spmm_bs(b200_ctx *ctx, const b200_csr *A, const T *X, int64_t ldx, T 
   // of X behind the first m_local ones -- the same aliasing make_xview does for the vector kernels
   const T *halo = A->halo ? (const T *)A->halo : X + A->m_local;
   const int64_t ldh = A->halo ? A->n_halo : ldx;
-#define LAUNCH(L)                                                                                                   \
-  k_spmm<T, L, BS><<<grid, kThreads, 0, ctx->stream>>>(A->rowptr, A->colind, (const T *)A->vals, X, ldx, halo, ldh, \
-                                                       (int)A->m_local, A->m_local, Y, ldy)
-  switch (lpr) {
-    case 2: LAUNCH(2); break;
-    case 4: LAUNCH(4); break;
-    case 8: LAUNCH(8); break;
-    case 16: LAUNCH(16); break;
-    default: LAUNCH(32); break;
-  }
-#undef LAUNCH
+  with_lpr<2>(lpr, [&](auto l) {
+    k_spmm<T, decltype(l)::value, BS><<<grid, kThreads, 0, ctx->stream>>>(
+        A->rowptr, A->colind, (const T *)A->vals, X, ldx, halo, ldh, (int)A->m_local, A->m_local, Y, ldy);
+  });
   B200_LAUNCH_CHECK(ctx);
   return B200_OK;
 }

@@ -6,6 +6,8 @@
 //
 // Algorithmic bytes per SpMV (SURVEY.md section 8d): nnz*(V+4) + (m+1)*4 + 2*m*V.
 #pragma once
+#include <type_traits>
+
 #include "csr.cuh"
 
 namespace b200 {
@@ -17,6 +19,16 @@ inline int pick_lpr(double avg_row_nnz) {
   int l = 2;
   while (l < 32 && l < avg_row_nnz) l <<= 1;
   return l;
+}
+
+// f(std::integral_constant<int, L>{}) for the compile-time lanes per row L == lpr, a power of two in [MIN, 32] (anything
+// else takes 32).  MIN keeps lane counts that no operator is given out of the instantiated kernels.
+template <int MIN, typename F>
+inline auto with_lpr(int lpr, F &&f) {
+  if constexpr (MIN < 32) {
+    if (lpr != MIN) return with_lpr<2 * MIN>(lpr, static_cast<F &&>(f));
+  }
+  return f(std::integral_constant<int, MIN>{});
 }
 
 // x gather from the extended vector: own slab or halo buffer
@@ -52,6 +64,26 @@ __device__ __forceinline__ T row_dot(const int *__restrict__ rowptr, const int *
 #pragma unroll
   for (int o = LPR >> 1; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o, LPR);
   return acc;
+}
+
+constexpr int kRowsThreads = 256;   // block size of the sub-warp form
+
+// Sub-warp (LPR lanes) per row over all rows; blocks stride the rows in interleaved chunks so that all resident blocks
+// work on neighbouring rows (keeps the x planes of a stencil matrix in L2).  The epilogue contract is the streamed
+// bodies' (spmv_stream.cuh): the lane that owns a row result calls epi.pre(row) and then epi(row, value, pre).
+template <typename T, int LPR, typename XV, typename Epi>
+__device__ __forceinline__ void spmv_rows(const int *__restrict__ rowptr, const int *__restrict__ colind,
+                                          const T *__restrict__ vals, const XV &xv, int64_t m, Epi &epi) {
+  constexpr int ROWS = kRowsThreads / LPR;
+  const int sub = threadIdx.x % LPR;
+  const int rib = threadIdx.x / LPR;
+  for (int64_t base = (int64_t)blockIdx.x * ROWS; base < m; base += (int64_t)gridDim.x * ROWS) {
+    const int64_t row = base + rib;
+    const bool own = row < m && sub == 0;
+    const T pre = own ? epi.pre(row) : (T)0;
+    const T v = row_dot<T, LPR>(rowptr, colind, vals, xv, row < m ? row : (m - 1), sub);
+    if (own) epi(row, v, pre);
+  }
 }
 
 #endif  // __CUDACC__

@@ -1,0 +1,89 @@
+// spmv_launch.cuh -- the three SpMV kernels and the one launch path shared by mul! (b200_spmv), cg!'s K2 and MINRES' Ka.
+//
+// A caller differs from the others only in its epilogue, a struct passed to the kernel by value:
+//   bool begin()                         all threads, before the body; false = the whole block returns (block-uniform)
+//   T pre(int64_t row)                   the epilogue's own per-row operand, requested ahead of the row's gathers
+//   void operator()(int64_t row, T v, T pre)   once per row, by the thread that owns the row result v = (A x)[row]
+//   template <int THREADS> void end(double *red)   all threads, after the body; red: THREADS / 32 doubles of shared memory
+//   bool rev()                           the streamed forms sweep the tiles from the last to the first (constexpr false
+//                                        where a caller never reverses, which keeps the sweep arithmetic out of its kernels)
+// Which of the three forms serves an operator is decided here alone (launch_spmv_fused).
+#pragma once
+#include "spmv_stream.cuh"
+
+namespace b200 {
+
+#ifdef __CUDACC__
+
+template <typename T, int LPR, typename Epi>
+__global__ void __launch_bounds__(kRowsThreads) k_spmv_rows(const int *__restrict__ rowptr, const int *__restrict__ colind,
+                                                            const T *__restrict__ vals, XView<T> xv, int64_t m, Epi epi) {
+  if (!epi.begin()) return;
+  __shared__ double red[kRowsThreads / 32];
+  spmv_rows<T, LPR>(rowptr, colind, vals, xv, m, epi);
+  epi.template end<kRowsThreads>(red);
+}
+
+template <typename T, int LPR, typename Epi>
+__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
+    k_spmv_csr_stream(const int *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
+                      XView<T> xv, int64_t m, Epi epi) {
+  if (!epi.begin()) return;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ double red[kStreamThreads / 32];
+  spmv_stream_tiles<T, LPR>(rowptr, colind, vals, xv, m, epi, reinterpret_cast<StreamSmem<T> *>(smem_raw), epi.rev());
+  epi.template end<kStreamThreads>(red);
+}
+
+template <typename T, typename Epi>
+__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
+    k_spmv_band_stream(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ x, int64_t nx, int64_t m, Epi epi) {
+  if (!epi.begin()) return;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ double red[kStreamThreads / 32];
+  spmv_band_tiles<T>(ba, vals, x, nx, m, epi, reinterpret_cast<BandSmem<T> *>(smem_raw), epi.rev());
+  epi.template end<kStreamThreads>(red);
+}
+
+// One launch of (A x)[row] -> epi over the local rows, in the form the operator and the option "spmv_kernel" select: the
+// band stream, the CSR stream, or the sub-warp form.  x is the operand of the local rows; peer_halo: the preceding halo
+// exchange filled A->halo_peer instead of A->halo.  chained: programmatic dependent launch (an epilogue that allows it
+// calls pdl_wait() in begin()).  Launches even when the operator has no local rows, so that a fused reduction in the
+// epilogue completes.
+template <typename T, typename Epi>
+int launch_spmv_fused(b200_ctx *ctx, const b200_csr *A, const void *x, bool peer_halo, const Epi &epi, bool chained) {
+  const T *vals = (const T *)A->vals;
+  const int64_t m = A->m_local;
+  if (use_band(ctx, A, x)) {
+    // band descriptions exist on single-GPU contexts only: x is the whole operand, n_global entries (== m for the
+    // square operators of the solvers)
+    const size_t smem = sizeof(BandSmem<T>);
+    B200_SMEM_ATTR_ONCE(ctx, smem, k_spmv_band_stream<T, Epi>);
+    B200_CUDA(launch_chained(chained, k_spmv_band_stream<T, Epi>, dim3(stream_grid_size(ctx, A)), dim3(kStreamThreads),
+                             smem, ctx->stream, make_band_args(A), vals, (const T *)x, A->n_global, m, epi));
+  } else if (use_stream(ctx, A)) {
+    const XView<T> xv = make_xview<T>(A, x, peer_halo);
+    const size_t smem = sizeof(StreamSmem<T>);
+    B200_TRY(with_lpr<1>(A->stream_lpr, [&](auto lpr) -> int {
+      constexpr int L = decltype(lpr)::value;
+      B200_SMEM_ATTR_ONCE(ctx, smem, k_spmv_csr_stream<T, L, Epi>);
+      B200_CUDA(launch_chained(chained, k_spmv_csr_stream<T, L, Epi>, dim3(stream_grid_size(ctx, A)),
+                               dim3(kStreamThreads), smem, ctx->stream, A->rowptr, A->colind, vals, xv, m, epi));
+      return B200_OK;
+    }));
+  } else {
+    const XView<T> xv = make_xview<T>(A, x, peer_halo);
+    B200_TRY(with_lpr<2>(pick_lpr(A->avg_row_nnz), [&](auto lpr) -> int {
+      constexpr int L = decltype(lpr)::value;
+      B200_CUDA(launch_chained(chained, k_spmv_rows<T, L, Epi>, dim3(stream_grid(ctx, m, kRowsThreads / L, 8)),
+                               dim3(kRowsThreads), 0, ctx->stream, A->rowptr, A->colind, vals, xv, m, epi));
+      return B200_OK;
+    }));
+  }
+  B200_LAUNCH_CHECK(ctx);
+  return B200_OK;
+}
+
+#endif  // __CUDACC__
+
+}  // namespace b200

@@ -17,9 +17,11 @@ SO = os.path.join(ROOT, "iterativesolvers.jl_b200", "libb200krylov.so")
 LOGS = os.path.join(ROOT, "iterativesolvers.jl_b200", "csrc", "build")
 OUT = os.path.join(ROOT, "profiles")
 
-# tag -> (substring of the mangled name that selects ONE instantiation, what to show)
+# tag -> (regular expression on the mangled name that selects ONE instantiation, what to show); the SpMV kernels'
+# epilogues live in anonymous namespaces, whose mangled names carry a per-file hash, hence the `.*`
 HOT = {
-    "cg_k2_spmv_dot_stream_f64": ("k_cg_spmv_dot_streamIdLi8E", "K2 of cg!: c = A u fused with dot(u, c); TMA-bulk streamed CSR"),
+    "cg_k2_spmv_dot_band_f64": (r"k_spmv_band_streamIdN.*8CgDotEpiIdE",
+                                "K2 of cg!: c = A u fused with dot(u, c); band stream (the form the Laplacian runs)"),
     "cg_persistent": ("k_cg_persistentIdLi8E", "cg! for small operators: the whole loop in one persistent cooperative kernel"),
     "cg_k1_update_u": ("k_cg_update_uId", "K1 of cg!: x += alpha u_old (deferred), u = r + beta u"),
     "cg_k3_update_r": ("k_cg_update_rId", "K3 of cg!: r -= alpha c fused with ||r||^2 (and the warp-parallel NVLink allreduce)"),
@@ -29,7 +31,8 @@ HOT = {
     "lobpcg_gram_wgmma": ("k_gram_wgmma", "LOBPCG Rayleigh-Ritz Gram products on wgmma"),
     "lobpcg_gram_legacy": ("k_gram_rr_tcILi2E", "LOBPCG Rayleigh-Ritz Gram products, legacy mma.sync path (kept for comparison)"),
     "pass_generic": ("k_passINS_8QmrWNextIdEE", "the fused-pass kernel of the general engines (one instantiation: QMR's w-recurrence pass)"),
-    "spmv_stream_f64": ("k_spmv_streamIdLi8E", "mul!(y, A, x): TMA-bulk streamed CSR SpMV"),
+    "spmv_csr_stream_f64": (r"k_spmv_csr_streamIdLi1EN.*8StoreEpiIdE",
+                            "mul!(y, A, x): TMA-bulk streamed CSR SpMV, one lane per row (the 7-point stencil's)"),
 }
 KEY = re.compile(r"\b(UBLKCP|UTMALDG|UTMASTG|SYNCS|HGMMA|UTC[A-Z]*MMA|UTCBAR|UTCCP|LDTM|STTM|UTCALLOC|HMMA|DFMA|DADD|DMUL|FFMA|"
                  r"LDG|STG|LDS|STS|REDG|ATOMG|SHFL|BAR|ACQBULK|ELECT|LDGSTS|CCTL|MEMBAR|ERRBAR|FENCE)\b")
@@ -77,7 +80,7 @@ def main():
     os.makedirs(OUT, exist_ok=True)
     written = []
     for tag, (needle, what) in HOT.items():
-        hits = [n for n in funcs if needle in n]
+        hits = [n for n in funcs if re.search(needle, n)]
         if not hits:
             continue
         n = sorted(hits, key=len)[0]
