@@ -16,6 +16,10 @@
     general   the general (callback-operator) engines of DESIGN sections 11 / 16 next to the tuned ones: cg!, minres! on
               laplace_matrix(Float64, N, 3), gmres!(30, CGS), bicgstabl!(2) on advection_dominated(N); the operator goes
               through the b200_linop interface with the library's own SpMV thunk (no host code inside the iteration)
+    complex   (command line only) ComplexF64 operators built on the host from laplace_matrix(Float64, N, 3)'s CSC arrays:
+              gmres!(30, CGS) on the shifted Helmholtz operator -Laplace - k^2 I + i sigma I, and cg! on the Hermitian
+              positive-definite L + I + i S (S the antisymmetric central difference in x, coefficient 1/4); fixed
+              iteration counts; one JSON line each with it/s, the complex SpMV's ms per launch and its GB/s
 
 Each line is a JSON object with iterations/s, per-kernel-class CUDA-event times recorded inside the run
 (b200_ctx_profile_*), the algorithmic bytes (SURVEY.md section 8d) and the achieved fraction of the measured
@@ -24,6 +28,7 @@ HBM peak.  Used for profiles/ (ncu launch lists are taken with the same commands
 import argparse
 import ctypes as C
 import json
+import math
 import os
 import sys
 import time
@@ -402,9 +407,83 @@ def run(which, grid=256, iters=None, orth="cgs", reps=2, ctx=None, clocks=True, 
     return out
 
 
+def gpu_name_power(device=0):
+    """the GPU's name and power limit (W) as nvidia-smi reports them: part of every number this script prints"""
+    import subprocess
+    try:
+        q = subprocess.run(["nvidia-smi", "-i", str(device), "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+        return {"gpu": q[0], "power_limit_w": q[1] if len(q) > 1 else None}
+    except Exception:
+        return {"gpu": None, "power_limit_w": None}
+
+
+def complex_operators(N, k2=0.5, sigma=0.5):
+    """ComplexF64 CSC arrays (colptr, rowval, nzval) of the shifted Helmholtz operator -Laplace - k^2 I + i sigma I and of
+    the Hermitian positive-definite L + I + i S, from laplace_matrix(Float64, N, 3) (0-based)."""
+    import iterativesolvers_jl_b200 as isb
+    colptr, rowval, nz, shape = isb.laplace_matrix(np.float64, N, 3, base=0)
+    col = np.repeat(np.arange(shape[1], dtype=np.int64), np.diff(colptr))
+    diag = rowval == col
+    helm = nz.astype(np.complex128)
+    helm[diag] += -k2 + 1j * sigma
+    hpd = nz.astype(np.complex128)
+    hpd[diag] += 1.0
+    hpd[col == rowval + 1] += 0.25j          # A[r, r+1] = -1 + i/4, A[r+1, r] = -1 - i/4: x-neighbours (stride 1)
+    hpd[col == rowval - 1] -= 0.25j
+    del col, diag
+    return colptr, rowval, helm, hpd, shape
+
+
+def run_complex(grid=256, iters=None, reps=2, ctx=None):
+    """the `complex` workloads: two records (gmres!(30) CGS on the Helmholtz operator, cg! on the HPD operator)"""
+    import iterativesolvers_jl_b200 as isb
+    ctx = ctx or isb.default_context()
+    L = isb.lib()
+    N = grid
+    n = N ** 3
+    colptr, rowval, helm, hpd, shape = complex_operators(N)
+    nnz = int(colptr[-1])
+    V = 16
+    spmv_b = nnz * (V + 4) + (n + 1) * 4 + 2 * n * V          # algorithmic bytes of one complex SpMV
+    gpu = gpu_name_power(ctx.device)
+    rng = np.random.default_rng(1234321)
+    b = (rng.standard_normal(n) + 1j * rng.standard_normal(n)) / math.sqrt(2 * n)
+    bd = isb.DeviceArray.from_numpy(ctx, b)
+    xd = isb.DeviceArray.zeros(ctx, n, np.complex128)
+    out = []
+    for name, vals in (("gmres", helm), ("cg", hpd)):
+        A = isb.B200CSR.from_csc_arrays(colptr, rowval, vals, shape, base=0, ctx=ctx)
+        it = iters or (90 if name == "gmres" else 200)
+        for rep in range(reps + 1):
+            L.b200_fill(ctx._h, n, 0.0, xd._p, isb._lib.CF64)
+            if rep == reps:
+                prof_reset(L, ctx)
+            ctx.sync()
+            t0 = time.perf_counter()
+            if name == "gmres":
+                x, h = isb.gmres_(xd, A, bd, restart=30, maxiter=it, orth_meth="cgs", initially_zero=True, log=True,
+                                  reltol=0.0)
+            else:
+                x, h = isb.cg_(xd, A, bd, maxiter=it, initially_zero=True, log=True, reltol=0.0)
+            ctx.sync()
+            dt = time.perf_counter() - t0
+        pr = prof_read(L, ctx)
+        sp_ms = pr["spmv_class"]["total_ms"] / max(pr["spmv_class"]["launches"], 1)
+        out.append({"config": "complex", "solver": "gmres!(restart=30, orth_meth=cgs), ComplexF64 Helmholtz" if name == "gmres"
+                    else "cg!, ComplexF64 Hermitian positive definite", "grid": N, "n": n, "nnz": nnz, **gpu,
+                    "iters": h.niters, "seconds": dt, "iters_per_s": h.niters / dt,
+                    "resnorm_first_last": [float(h["resnorm"][0]), float(h["resnorm"][-1])],
+                    "spmv_ms_per_launch": sp_ms, "spmv_bytes": spmv_b, "spmv_gbs": spmv_b / (sp_ms * 1e-3) / 1e9,
+                    "spmv_frac_of_3350_gbs": spmv_b / (sp_ms * 1e-3) / 1e9 / 3350.0, "profile": pr})
+        A.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("which", choices=["gmres", "lobpcg", "minres", "bicgstabl", "cg256", "widen", "general", "scattered", "cg2d"])
+    ap.add_argument("which", choices=["gmres", "lobpcg", "minres", "bicgstabl", "cg256", "widen", "general", "scattered", "cg2d",
+                                      "complex"])
     ap.add_argument("--grid", type=int, default=256)
     ap.add_argument("--iters", type=int, default=None)
     ap.add_argument("--orth", default="cgs")
@@ -414,6 +493,10 @@ def main():
     args = ap.parse_args()
     import torch
     torch.cuda.set_device(0)
+    if args.which == "complex":
+        for rec in run_complex(args.grid, args.iters, args.reps):
+            print(json.dumps(rec))
+        return
     print(json.dumps(run(args.which, args.grid, args.iters, args.orth, args.reps, clocks=not args.no_clocks, solves=args.solves)))
 
 

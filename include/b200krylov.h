@@ -14,7 +14,13 @@
  *     nothing throws, nothing calls exit().  Non-convergence is NOT an error (reference
  *     src/cg.jl:238): it is reported through b200_result.isconverged.
  *   - all device work is ordered on the context's CUDA stream; one host thread per context.
- *   - `dtype`: B200_F64 or B200_F32 (the configs of BASELINE.json need no complex types).
+ *   - `dtype`: B200_F64, B200_F32, B200_CF64 (ComplexF64) or B200_CF32 (ComplexF32).  Complex values are
+ *     interleaved (re, im) pairs -- the layout of Julia's Complex{T} and numpy's complex128 / complex64 -- aligned
+ *     to the real component only (8 bytes for ComplexF64): views at any element offset are accepted.  Complex
+ *     element types are served by b200_csr_from_csc / _info / _download / _diag / _stream_kind / _as_linop,
+ *     b200_spmv, the BLAS-1 calls (b200_dotc instead of b200_dot), b200_cg_solve[_host|_op] and
+ *     b200_gmres_solve[_op], on single-GPU contexts.  Every other entry point returns B200_ERR_UNSUPPORTED for a
+ *     complex operator or dtype before it touches any data.
  *   - device pointers are raw CUDA device addresses (cudaMalloc / torch tensor .data_ptr()).
  *   - there is NO CPU fallback: without a CUDA device every compute entry point fails with
  *     B200_ERR_CUDA.
@@ -31,7 +37,7 @@ extern "C" {
 
 #define B200_API __attribute__((visibility("default")))
 
-enum { B200_F64 = 0, B200_F32 = 1 };
+enum { B200_F64 = 0, B200_F32 = 1, B200_CF64 = 2 /* ComplexF64 */, B200_CF32 = 3 /* ComplexF32 */ };
 
 enum {
   B200_OK = 0,
@@ -116,7 +122,7 @@ B200_API int b200_ctx_profile_read(b200_ctx *ctx, int slot, double *total_ms, in
  *           else the CSR stream when the tiles fit, else sub-warp per row), 1 = sub-warp-per-row kernel,
  *           2 = TMA-streamed CSR kernel (when the tiles fit), 3 = band stream (when the operator has a band
  *           description and x is 16-byte aligned, else as 0).  The band stream and the CSR stream give
- *           bit-identical results
+ *           bit-identical results.  Complex operators always take the sub-warp form
  *   "snake": 1 (default) = consecutive hot kernels of a solver sweep the rows in alternating directions so
  *           that each starts on the data the previous one touched last (L2 reuse); 0 = always ascending
  *   "orth_fused": 1 (default) = orthogonalize_and_normalize! (CGS / DGKS) is ONE cooperative launch (dots, update, norm,
@@ -182,7 +188,7 @@ B200_API int b200_csr_transpose(b200_ctx *ctx, const b200_csr *A, b200_csr **out
 /* Which form of the streamed SpMV the operator got when it was built (the form "spmv_kernel" = 0 selects):
  * kind 3 = band stream (a single-GPU operator whose 512-row tiles each have at most 8 distinct diagonal offsets
  * col - row and whose rows have strictly ascending columns: per tile its offsets, per row one mask byte),
- * 2 = CSR stream, 1 = sub-warp-per-row kernel.  structure_bytes = bytes of structure (everything but vals and the
+ * 2 = CSR stream, 1 = sub-warp-per-row kernel (always for complex operators).  structure_bytes = bytes of structure (everything but vals and the
  * vectors) that form reads per SpMV: 576 per 512-row tile for the band stream, 4*nnz + 4*(rows+1) for CSR. */
 B200_API int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes);
 /* diag(A) of the local rows into a device vector (JacobiPrec(diag(A)), reference test/cg.jl:57) */
@@ -246,10 +252,14 @@ B200_API int b200_spmv(b200_ctx *ctx, const b200_csr *A, const void *x_dev, void
 /* mul!(Y, A, X) on column-major m x bs blocks (reference src/lobpcg.jl:124-131) */
 B200_API int b200_spmm(b200_ctx *ctx, const b200_csr *A, const void *X_dev, int64_t ldx, void *Y_dev, int64_t ldy,
                        int bs);
-/* dot(x, y), norm(x) (host result, synchronises) */
+/* dot(x, y), norm(x) (host result, synchronises).  b200_dot is real-only; norm(x) = sqrt(sum |x_i|^2) for every dtype */
 B200_API int b200_dot(b200_ctx *ctx, int64_t n, const void *x_dev, const void *y_dev, int dtype, double *result);
+/* dot(x, y) = sum conj(x_i) y_i for complex vectors (Julia's dot): result[0] = real part, result[1] = imaginary part.
+ * Real dtypes are accepted too (result[1] = 0).  The reduction is as deterministic as b200_dot's. */
+B200_API int b200_dotc(b200_ctx *ctx, int64_t n, const void *x_dev, const void *y_dev, int dtype, double result[2]);
 B200_API int b200_nrm2(b200_ctx *ctx, int64_t n, const void *x_dev, int dtype, double *result);
-/* y .= a .* x .+ b .* y  (axpy!: b=1; broadcast update of src/cg.jl:51: a=1,x=r,b=beta) */
+/* y .= a .* x .+ b .* y  (axpy!: b=1; broadcast update of src/cg.jl:51: a=1,x=r,b=beta).  The scalars are real for
+ * every dtype; b200_fill sets (a, 0) on complex vectors */
 B200_API int b200_axpby(b200_ctx *ctx, int64_t n, double a, const void *x_dev, double b, void *y_dev, int dtype);
 B200_API int b200_scal(b200_ctx *ctx, int64_t n, double a, void *x_dev, int dtype);           /* rmul! */
 B200_API int b200_copy(b200_ctx *ctx, int64_t n, const void *x_dev, void *y_dev, int dtype);  /* copyto! */

@@ -37,10 +37,15 @@ default_ctx() = something(DEFAULT_CTX[], (DEFAULT_CTX[] = Ctx(0)))
 
 dtype_code(::Type{Float64}) = Cint(0)
 dtype_code(::Type{Float32}) = Cint(1)
+dtype_code(::Type{ComplexF64}) = Cint(2)   # interleaved (re, im): Complex{T}'s own memory layout
+dtype_code(::Type{ComplexF32}) = Cint(3)
 const BlasReal = Union{Float32,Float64}
+# element types of device vectors and operators; complex ones are served by mul!, the BLAS-1 calls, cg! and gmres!
+# (the other entry points return B200_ERR_UNSUPPORTED for them)
+const B200Eltype = Union{Float32,Float64,ComplexF32,ComplexF64}
 
 # ------------------------------------------------------------------------------------------- vectors
-mutable struct B200Vector{T<:BlasReal} <: AbstractVector{T}
+mutable struct B200Vector{T<:B200Eltype} <: AbstractVector{T}
     p::Ptr{T}
     n::Int
     ctx::Ctx
@@ -55,7 +60,7 @@ mutable struct B200Vector{T<:BlasReal} <: AbstractVector{T}
 end
 Base.size(v::B200Vector) = (v.n,)
 Base.similar(v::B200Vector{T}) where {T} = B200Vector{T}(v.ctx, v.n)
-function B200Vector(ctx::Ctx, x::Vector{T}) where {T<:BlasReal}
+function B200Vector(ctx::Ctx, x::Vector{T}) where {T<:B200Eltype}
     v = B200Vector{T}(ctx, length(x))
     check(ccall((:b200_upload, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Csize_t), ctx.h, v.p, x, sizeof(x)))
     v
@@ -67,12 +72,16 @@ function Base.Array(v::B200Vector{T}) where {T}
 end
 # operator-level BLAS-1: lets the UNMODIFIED reference loops (src/cg.jl:43-66, src/minres.jl:97-159) run on
 # device vectors, one ccall per Julia operation
-LinearAlgebra.dot(x::B200Vector{T}, y::B200Vector{T}) where {T} = (r = Ref{Cdouble}();
+LinearAlgebra.dot(x::B200Vector{T}, y::B200Vector{T}) where {T<:BlasReal} = (r = Ref{Cdouble}();
     check(ccall((:b200_dot, LIB), Cint, (Ptr{Cvoid}, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ref{Cdouble}),
                 x.ctx.h, x.n, x.p, y.p, dtype_code(T), r)); T(r[]))
+# dot(x, y) = sum(conj(x) .* y) for complex vectors
+LinearAlgebra.dot(x::B200Vector{T}, y::B200Vector{T}) where {T<:Union{ComplexF32,ComplexF64}} = (r = zeros(Cdouble, 2);
+    check(ccall((:b200_dotc, LIB), Cint, (Ptr{Cvoid}, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Cint, Ptr{Cdouble}),
+                x.ctx.h, x.n, x.p, y.p, dtype_code(T), r)); T(complex(r[1], r[2])))
 LinearAlgebra.norm(x::B200Vector{T}) where {T} = (r = Ref{Cdouble}();
     check(ccall((:b200_nrm2, LIB), Cint, (Ptr{Cvoid}, Int64, Ptr{Cvoid}, Cint, Ref{Cdouble}),
-                x.ctx.h, x.n, x.p, dtype_code(T), r)); T(r[]))
+                x.ctx.h, x.n, x.p, dtype_code(T), r)); real(T)(r[]))
 # y = a*x + b*y
 axpby!(a, x::B200Vector{T}, b, y::B200Vector{T}) where {T} =
     (check(ccall((:b200_axpby, LIB), Cint, (Ptr{Cvoid}, Int64, Cdouble, Ptr{Cvoid}, Cdouble, Ptr{Cvoid}, Cint),
@@ -86,7 +95,7 @@ Base.fill!(x::B200Vector{T}, a::Number) where {T} =
     (check(ccall((:b200_fill, LIB), Cint, (Ptr{Cvoid}, Int64, Cdouble, Ptr{Cvoid}, Cint), x.ctx.h, x.n, a, x.p, dtype_code(T))); x)
 
 # ------------------------------------------------------------------------------------------- operator
-mutable struct B200CSR{T<:BlasReal}
+mutable struct B200CSR{T<:B200Eltype}
     h::Ptr{Cvoid}
     ctx::Ctx
     n::Int                                  # size(A, 1)
@@ -94,7 +103,7 @@ mutable struct B200CSR{T<:BlasReal}
     adj::Union{Nothing,B200CSR{T}}          # adjoint(A), built on first use
 end
 # stands where a SparseMatrixCSC is passed today (src/cg.jl:54, src/gmres.jl:287, ...): CSC -> device CSR int32
-function B200CSR(A::SparseMatrixCSC{T,Ti}; ctx::Ctx = default_ctx()) where {T<:BlasReal,Ti<:Union{Int32,Int64}}
+function B200CSR(A::SparseMatrixCSC{T,Ti}; ctx::Ctx = default_ctx()) where {T<:B200Eltype,Ti<:Union{Int32,Int64}}
     r = Ref{Ptr{Cvoid}}()
     check(ccall((:b200_csr_from_csc, LIB), Cint,
                 (Ptr{Cvoid}, Int64, Int64, Ptr{Ti}, Ptr{Ti}, Ptr{T}, Cint, Cint, Cint, Ref{Ptr{Cvoid}}),
@@ -215,7 +224,7 @@ end
 
 # ------------------------------------------------------------------------------------------- cg!
 function cg!(x::B200Vector{T}, A::B200CSR{T}, b::B200Vector{T};
-             abstol::Real = zero(T), reltol::Real = sqrt(eps(T)), maxiter::Int = size(A, 2), log::Bool = false,
+             abstol::Real = zero(real(T)), reltol::Real = sqrt(eps(real(T))), maxiter::Int = size(A, 2), log::Bool = false,
              verbose::Bool = false, Pl = Identity(), initially_zero::Bool = false, kwargs...) where {T}
     res = Result(); hist = Vector{Float64}(undef, log ? maxiter + 1 : 0)
     o = CgOpts(abstol, reltol, maxiter, initially_zero, 0, prec(Pl), 0, 0)
@@ -226,7 +235,7 @@ function cg!(x::B200Vector{T}, A::B200CSR{T}, b::B200Vector{T};
 end
 # host arrays: one call does H2D of b and x, the solve, D2H of x
 function cg!(x::Vector{T}, A::B200CSR{T}, b::Vector{T};
-             abstol::Real = zero(T), reltol::Real = sqrt(eps(T)), maxiter::Int = size(A, 2), log::Bool = false,
+             abstol::Real = zero(real(T)), reltol::Real = sqrt(eps(real(T))), maxiter::Int = size(A, 2), log::Bool = false,
              verbose::Bool = false, Pl = Identity(), initially_zero::Bool = false, kwargs...) where {T}
     res = Result(); hist = Vector{Float64}(undef, log ? maxiter + 1 : 0)
     o = CgOpts(abstol, reltol, maxiter, initially_zero, 0, prec(Pl), 0, 0)
@@ -279,7 +288,7 @@ end
 
 # ------------------------------------------------------------------------------------------- gmres!
 function gmres!(x::Vector{T}, A::B200CSR{T}, b::Vector{T};
-                Pl = Identity(), Pr = Identity(), abstol::Real = zero(T), reltol::Real = sqrt(eps(T)),
+                Pl = Identity(), Pr = Identity(), abstol::Real = zero(real(T)), reltol::Real = sqrt(eps(real(T))),
                 restart::Int = min(20, size(A, 2)), maxiter::Int = size(A, 2), log::Bool = false,
                 initially_zero::Bool = false, verbose::Bool = false,
                 orth_meth::OrthogonalizationMethod = ModifiedGramSchmidt()) where {T}
@@ -538,7 +547,7 @@ linop(op::B200LinearOperator{T}) where {T} =
           op.m, op.n, op.n, op.m, dtype_code(T), 0)
 
 function cg!(x::B200Vector{T}, A::B200LinearOperator{T}, b::B200Vector{T};
-             abstol::Real = zero(T), reltol::Real = sqrt(eps(T)), maxiter::Int = A.n, log::Bool = false,
+             abstol::Real = zero(real(T)), reltol::Real = sqrt(eps(real(T))), maxiter::Int = A.n, log::Bool = false,
              Pl = Identity(), initially_zero::Bool = false, verbose::Bool = false) where {T}
     res = Result(); hist = Vector{Float64}(undef, log ? maxiter + 1 : 0)
     cb = Pl isa B200LinearOperator                                         # ldiv!(c, Pl, r) by callback
@@ -567,7 +576,7 @@ end
 
 # gmres!(x, A, b; Pl, Pr, ...) with `mul!` / `ldiv!` callbacks  src/gmres.jl:184-194 (expand! :285-304)
 function gmres!(x::B200Vector{T}, A::Union{B200CSR{T},B200LinearOperator{T}}, b::B200Vector{T};
-                Pl = Identity(), Pr = Identity(), abstol::Real = zero(T), reltol::Real = sqrt(eps(T)),
+                Pl = Identity(), Pr = Identity(), abstol::Real = zero(real(T)), reltol::Real = sqrt(eps(real(T))),
                 restart::Int = min(20, size(A, 2)), maxiter::Int = size(A, 2), log::Bool = false,
                 initially_zero::Bool = false, verbose::Bool = false,
                 orth_meth::OrthogonalizationMethod = ModifiedGramSchmidt()) where {T}

@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.path.join(_HERE, "libb200krylov.so")
 
 F64, F32 = 0, 1
+CF64, CF32 = 2, 3          # ComplexF64, ComplexF32: interleaved (re, im), numpy complex128 / complex64
 ORTH_MGS, ORTH_CGS, ORTH_DGKS = 0, 1, 2
 PREC_IDENTITY, PREC_JACOBI, PREC_CALLBACK = 0, 1, 2
 ERR_INVALID = -1
@@ -172,6 +173,7 @@ SIGNATURES = {
     "b200_spmv": (_INT, [_P, _P, _P, _P]),
     "b200_spmm": (_INT, [_P, _P, _P, _I64, _P, _I64, _INT]),
     "b200_dot": (_INT, [_P, _I64, _P, _P, _INT, C.POINTER(_DBL)]),
+    "b200_dotc": (_INT, [_P, _I64, _P, _P, _INT, C.POINTER(_DBL)]),
     "b200_nrm2": (_INT, [_P, _I64, _P, _INT, C.POINTER(_DBL)]),
     "b200_axpby": (_INT, [_P, _I64, _DBL, _P, _DBL, _P, _INT]),
     "b200_scal": (_INT, [_P, _I64, _DBL, _P, _INT]),

@@ -10,6 +10,7 @@ namespace b200 {
 int spmv(b200_ctx *ctx, const b200_csr *A, const void *x, void *y);  // halo exchange + y = A x
 int spmv_gated(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate, int gate_mask);   // world == 1
 int dot_dev(b200_ctx *ctx, int64_t n, const void *x, const void *y, int dtype, double *out_dev);
+int dotc_dev(b200_ctx *ctx, int64_t n, const void *x, const void *y, int dtype, double *out_dev);   // complex: 2 doubles
 int allreduce_sum_dev(b200_ctx *ctx, double *buf_dev, int count);
 int read_scalars(b200_ctx *ctx, const double *src_dev, int count, double *dst_host);
 int axpby(b200_ctx *ctx, int64_t n, double a, const void *x, double b, void *y, int dtype);

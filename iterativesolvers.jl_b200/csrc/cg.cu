@@ -842,7 +842,8 @@ extern "C" {
 
 int b200_cg_solve(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *b_dev, const b200_cg_opts *opts,
                   b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
-  if (ctx && A && x_dev && b_dev && opts && opts->Pl.kind == B200_PREC_CALLBACK) {   // ldiv! by callback: the general engine
+  // ldiv! by callback, or a complex operator (the tuned engine below is real-only): the general engine
+  if (ctx && A && x_dev && b_dev && opts && (opts->Pl.kind == B200_PREC_CALLBACK || is_complex_dtype(A->dtype))) {
     B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
     B200_REQUIRE(is_square(A), "this solver needs a square operator");
     return cg_general(ctx, CudaOp{A, nullptr}, A->dtype, A->m_local, A->n_global, nullptr, x_dev, b_dev, opts, res,
@@ -880,6 +881,7 @@ struct b200_cg_iter {
 
 int b200_cg_iter_create(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *b_dev, const b200_cg_opts *opts,
                         void *u_dev, void *r_dev, void *c_dev, b200_cg_iter **out) {
+  B200_TRY(real_only(A, "b200_cg_iter_create"));
   B200_TRY(check_cg_args(ctx, A, x_dev, b_dev, opts));
   B200_REQUIRE(out, "NULL argument");
   B200_CUDA(cudaSetDevice(ctx->device));

@@ -13,7 +13,12 @@
 //   C3  x += alpha u ; r -= alpha c ; residual = ||r||    S, C2 (alpha = rho / <u, c>), C3                          :89-96
 //                                       :58-62
 // Algorithmic bytes per iteration besides the operator: CG 3 + 2 + 5 = 10 n V, PCG (Jacobi) 3 + 3 + 2 + 5 = 13 n V.
+//
+// Complex element types (T = cplx<R>): the scalar block is CgpScalC, where alpha, rho and beta are complex (fp64 for
+// ComplexF32 too) and residual stays real; every dot is Julia's dot(x, y) = sum conj(x_i) y_i and takes two of a pass's
+// sums (re, im).  The real instantiations are the code they were before complex types existed (if constexpr).
 #pragma once
+#include "complex.h"
 #include "pass_core.h"
 
 namespace b200 {
@@ -28,7 +33,29 @@ struct CgpScal {
   int done, breakdown, precond, pad;
 };
 
-B200_HD void cgp_publish(CgpScal *q, double residual) {       // after :62 / :96
+// complex element types: alpha, rho, beta complex (src/cg.jl:55, :82, :85), residual real
+struct CgpScalC {
+  double residual, prev_residual;
+  cplx<double> rho;
+  double tol, abstol, reltol;
+  cplx<double> alpha, beta;
+  double sum[2];
+  double *hist;
+  long long hist_cap, n_hist;
+  long long iteration, maxiter;
+  int done, breakdown, precond, pad;
+};
+template <typename T>
+struct cgp_scal {
+  typedef CgpScal type;
+};
+template <typename R>
+struct cgp_scal<cplx<R>> {
+  typedef CgpScalC type;
+};
+
+template <typename Q>
+B200_HD void cgp_publish(Q *q, double residual) {             // after :62 / :96
   q->residual = residual;
   if (!(residual == residual)) q->breakdown = 1;
   if (q->hist && q->n_hist < q->hist_cap) q->hist[q->n_hist] = residual;
@@ -40,10 +67,11 @@ B200_HD void cgp_publish(CgpScal *q, double residual) {       // after :62 / :96
 // ---- cg_iterator! :126-141
 template <typename T>
 struct CgpInit {
+  typedef typename cgp_scal<T>::type Scal;
   static constexpr int NRED = 1;
   const T *b, *ax;       // ax = A*x (nullptr when initially_zero)
   T *r, *u;
-  CgpScal *s;
+  Scal *s;
   B200_HD bool skip() const { return false; }
   B200_HD void load() {}
   B200_HD void elem(int64_t i, double *acc) const {
@@ -51,11 +79,12 @@ struct CgpInit {
     if (ax) ri = ri - ax[i];                           // r .-= c :138
     r[i] = ri;
     u[i] = (T)0;                                       // :129
-    acc[0] += (double)ri * (double)ri;
+    if constexpr (is_cplx<T>::value) acc[0] += (double)ri.re * (double)ri.re + (double)ri.im * (double)ri.im;
+    else acc[0] += (double)ri * (double)ri;
   }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
-    CgpScal *q = s;
+    Scal *q = s;
     q->residual = sqrt(tot[0]);                        // :140
     q->tol = fmax(q->reltol * q->residual, q->abstol); // :141
     q->prev_residual = 1.0;                            // one(residual) :146
@@ -74,7 +103,7 @@ struct CgpUpdateU {
   static constexpr int NRED = 0;
   const T *z;
   T *u;
-  const CgpScal *s;
+  const typename cgp_scal<T>::type *s;
   T beta;
   B200_HD bool skip() const { return s->done != 0; }
   B200_HD void load() { beta = (T)s->beta; }
@@ -86,10 +115,10 @@ struct CgpUpdateU {
 // ---- D: rho = <c, r> (PCG).  With a Jacobi preconditioner the pass also forms c = r ./ d.
 template <typename T>
 struct CgpRho {
-  static constexpr int NRED = 1;
+  static constexpr int NRED = is_cplx<T>::value ? 2 : 1;
   T *c;
   const T *r, *diag;     // diag: Jacobi (c is written here); nullptr: c was produced by the preconditioner callback
-  CgpScal *s;
+  typename cgp_scal<T>::type *s;
   B200_HD bool skip() const { return s->done != 0; }
   B200_HD void load() {}
   B200_HD void elem(int64_t i, double *acc) const {
@@ -101,38 +130,61 @@ struct CgpRho {
     } else {
       ci = c[i];
     }
-    acc[0] += (double)ci * (double)ri;                 // dot(c, r) :82
+    if constexpr (is_cplx<T>::value) {                 // dot(c, r) = sum conj(c_i) r_i :82
+      acc[0] += (double)ci.re * (double)ri.re + (double)ci.im * (double)ri.im;
+      acc[1] += (double)ci.re * (double)ri.im - (double)ci.im * (double)ri.re;
+    } else {
+      acc[0] += (double)ci * (double)ri;               // dot(c, r) :82
+    }
   }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
-    const double rho_prev = s->rho;                    // :81
-    s->rho = tot[0];                                   // :82
-    s->beta = s->rho / rho_prev;                       // :85
+    if constexpr (is_cplx<T>::value) {
+      const cplx<double> rho_prev = s->rho;            // :81
+      s->rho = cplx<double>(tot[0], tot[1]);           // :82
+      s->beta = s->rho / rho_prev;                     // :85
+    } else {
+      const double rho_prev = s->rho;                  // :81
+      s->rho = tot[0];                                 // :82
+      s->beta = s->rho / rho_prev;                     // :85
+    }
   }
 };
 
 // ---- C2: alpha
 template <typename T>
 struct CgpAlpha {
-  static constexpr int NRED = 1;
+  static constexpr int NRED = is_cplx<T>::value ? 2 : 1;
   const T *u, *c;
-  CgpScal *s;
+  typename cgp_scal<T>::type *s;
   B200_HD bool skip() const { return s->done != 0; }
   B200_HD void load() {}
-  B200_HD void elem(int64_t i, double *acc) const { acc[0] += (double)u[i] * (double)c[i]; }
+  B200_HD void elem(int64_t i, double *acc) const {
+    if constexpr (is_cplx<T>::value) {                 // dot(u, c) = sum conj(u_i) c_i
+      const T ui = u[i], ci = c[i];
+      acc[0] += (double)ui.re * (double)ci.re + (double)ui.im * (double)ci.im;
+      acc[1] += (double)ui.re * (double)ci.im - (double)ui.im * (double)ci.re;
+    } else {
+      acc[0] += (double)u[i] * (double)c[i];
+    }
+  }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
-    s->alpha = (s->precond ? s->rho : s->residual * s->residual) / tot[0];   // :90 / :55
+    if constexpr (is_cplx<T>::value)
+      s->alpha = (s->precond ? s->rho : cplx<double>(s->residual * s->residual)) / cplx<double>(tot[0], tot[1]);
+    else
+      s->alpha = (s->precond ? s->rho : s->residual * s->residual) / tot[0];   // :90 / :55
   }
 };
 
 // ---- C3
 template <typename T>
 struct CgpUpdateXR {
+  typedef typename cgp_scal<T>::type Scal;
   static constexpr int NRED = 1;
   T *x, *r;
   const T *u, *c;
-  CgpScal *s;
+  Scal *s;
   T alpha;
   B200_HD bool skip() const { return s->done != 0; }
   B200_HD void load() { alpha = (T)s->alpha; }
@@ -140,11 +192,12 @@ struct CgpUpdateXR {
     x[i] = x[i] + alpha * u[i];                        // :58 / :93
     const T ri = r[i] - alpha * c[i];                  // :59 / :94
     r[i] = ri;
-    acc[0] += (double)ri * (double)ri;
+    if constexpr (is_cplx<T>::value) acc[0] += (double)ri.re * (double)ri.re + (double)ri.im * (double)ri.im;
+    else acc[0] += (double)ri * (double)ri;
   }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
-    CgpScal *q = s;
+    Scal *q = s;
     const double res = sqrt(tot[0]);                   // :62 / :96
     if (!q->precond) {
       q->prev_residual = q->residual;                  // :61
@@ -165,7 +218,7 @@ struct CgpOutcome {
 template <typename T>
 struct CgpLayout {
   T *u, *r, *c;
-  CgpScal *s;
+  typename cgp_scal<T>::type *s;
   double *hist;
   int64_t hist_cap;
 };
@@ -176,14 +229,14 @@ size_t cgp_ws_bytes(int64_t n, int64_t hist_cap) {
 }
 template <typename T>
 CgpLayout<T> cgp_layout(void *ws, int64_t n, int64_t hist_cap) {
-  static_assert(sizeof(CgpScal) <= 512, "CgpScal outgrew its slot");
+  static_assert(sizeof(CgpScal) <= 512 && sizeof(CgpScalC) <= 512, "CgpScal outgrew its slot");
   const size_t vb = cgp_vec_bytes(sizeof(T), n);
   CgpLayout<T> L;
   char *p = (char *)ws;
   L.u = (T *)p; p += vb;
   L.r = (T *)p; p += vb;
   L.c = (T *)p; p += vb;
-  L.s = (CgpScal *)p; p += 512;
+  L.s = (typename cgp_scal<T>::type *)p; p += 512;
   L.hist = hist_cap > 0 ? (double *)p : nullptr;
   L.hist_cap = hist_cap > 0 ? hist_cap : 0;
   return L;
@@ -196,7 +249,7 @@ int cgp_setup(B &be, const typename B::Op *A, bool precond, const CgpLayout<T> &
               const T *b, double abstol, double reltol, int64_t maxiter, int initially_zero, int64_t *mvps0) {
   if (reltol < 0) reltol = sqrt(eps_of<T>());                               // :211
   if (maxiter < 0) maxiter = n_global;                                      // :212
-  CgpScal h;
+  typename cgp_scal<T>::type h;
   memset(&h, 0, sizeof(h));
   h.abstol = abstol;
   h.reltol = reltol;
@@ -220,8 +273,8 @@ int cgp_advance(B &be, const typename B::Op *A, const typename B::Op *Pl, const 
                 T *x, int64_t k, int check_every) {
   int st;
   T *u = L.u, *r = L.r, *c = L.c;
-  CgpScal *s = L.s;
-  CgpScal h;
+  typename cgp_scal<T>::type *s = L.s;
+  typename cgp_scal<T>::type h;
   if ((st = be.to_host(&h, s, sizeof(h)))) return st;
   if (h.done) return 0;
   const bool precond = Pl != nullptr || diag != nullptr;
@@ -254,7 +307,7 @@ int cgp_advance(B &be, const typename B::Op *A, const typename B::Op *Pl, const 
 template <typename T, typename B>
 int cgp_collect(B &be, const CgpLayout<T> &L, int64_t mvps0, double *hist_host, CgpOutcome *out) {
   int st;
-  CgpScal h;
+  typename cgp_scal<T>::type h;
   if ((st = be.to_host(&h, L.s, sizeof(h)))) return st;
   out->iters = h.iteration;
   out->mvps = mvps0 + h.iteration;
@@ -267,8 +320,8 @@ int cgp_collect(B &be, const CgpLayout<T> &L, int64_t mvps0, double *hist_host, 
   if (hist_host && out->n_hist > 0 && (st = be.to_host(hist_host, L.hist, sizeof(double) * (size_t)out->n_hist))) return st;
   return 0;
 }
-template <typename B>
-int cgp_reset_window(B &be, CgpScal *s) {
+template <typename B, typename Q>
+int cgp_reset_window(B &be, Q *s) {
   const long long zero = 0;
   return be.to_device(&s->n_hist, &zero, sizeof(zero));
 }

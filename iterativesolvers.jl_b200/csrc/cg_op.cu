@@ -15,8 +15,12 @@ namespace b200 {
 int cg_general(b200_ctx *ctx, const CudaOp &A, int dtype, int64_t n, int64_t n_global, const b200_linop *Pl, void *x_dev,
                const void *b_dev, const b200_cg_opts *opts, b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
   if (!Pl && opts->Pl.kind == B200_PREC_CALLBACK) Pl = (const b200_linop *)opts->Pl.diag;
+  if (is_complex_dtype(dtype) && ctx->world > 1) {
+    set_error("cg!: %s operators are single-GPU in this version", dtype_name(dtype));
+    return B200_ERR_UNSUPPORTED;
+  }
   if (Pl) {
-    B200_TRY(check_linop(Pl, "Pl"));
+    B200_TRY(check_linop_complex(Pl, "Pl"));
     B200_REQUIRE(Pl->dtype == dtype && Pl->m_local == n && Pl->n_local == n,
                  "Pl must act on vectors of the operator's local length");
   } else {
@@ -30,7 +34,17 @@ int cg_general(b200_ctx *ctx, const CudaOp &A, int dtype, int64_t n, int64_t n_g
   const void *diag = (!Pl && opts->Pl.kind == B200_PREC_JACOBI) ? opts->Pl.diag : nullptr;
   CgpOutcome o;
   memset(&o, 0, sizeof(o));
-  const int st = dtype == B200_F64
+  int st;
+  if (dtype == B200_CF64)
+    st = cgp_run<cplx<double>>(be, &A, Pl ? &p : nullptr, (const cplx<double> *)diag, n, n_global, (cplx<double> *)x_dev,
+                               (const cplx<double> *)b_dev, opts->abstol, opts->reltol, opts->maxiter, opts->initially_zero,
+                               opts->check_every, resnorm_cap, resnorm_host, &o);
+  else if (dtype == B200_CF32)
+    st = cgp_run<cplx<float>>(be, &A, Pl ? &p : nullptr, (const cplx<float> *)diag, n, n_global, (cplx<float> *)x_dev,
+                              (const cplx<float> *)b_dev, opts->abstol, opts->reltol, opts->maxiter, opts->initially_zero,
+                              opts->check_every, resnorm_cap, resnorm_host, &o);
+  else
+    st = dtype == B200_F64
                      ? cgp_run<double>(be, &A, Pl ? &p : nullptr, (const double *)diag, n, n_global, (double *)x_dev,
                                        (const double *)b_dev, opts->abstol, opts->reltol, opts->maxiter,
                                        opts->initially_zero, opts->check_every, resnorm_cap, resnorm_host, &o)
@@ -101,6 +115,7 @@ extern "C" {
 int b200_chebyshev_solve_op(b200_ctx *ctx, const b200_linop *A, void *x_dev, const void *b_dev, double lambda_min,
                             double lambda_max, const b200_cg_opts *opts, b200_result *res, double *resnorm_host,
                             int64_t resnorm_cap) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_chebyshev_solve_op"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts, "NULL argument");
   B200_TRY(check_linop(A, "A"));
   B200_REQUIRE(A->m_global == A->n_global && A->m_local == A->n_local, "chebyshev! needs a square operator");
@@ -111,7 +126,7 @@ int b200_chebyshev_solve_op(b200_ctx *ctx, const b200_linop *A, void *x_dev, con
 int b200_cg_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *Pl, void *x_dev, const void *b_dev,
                      const b200_cg_opts *opts, b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
   B200_REQUIRE(ctx && x_dev && b_dev && opts, "NULL argument");
-  B200_TRY(check_linop(A, "A"));
+  B200_TRY(check_linop_complex(A, "A"));
   B200_REQUIRE(A->m_global == A->n_global && A->m_local == A->n_local, "cg! needs a square operator");
   return cg_general(ctx, CudaOp{nullptr, A}, A->dtype, A->m_local, A->n_global, Pl, x_dev, b_dev, opts, res, resnorm_host,
                     resnorm_cap);
@@ -121,6 +136,8 @@ int b200_cg_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *Pl, v
 // and Aop (callback: e.g. the action of inv(A - shift I) for inverse iteration) is non-NULL.
 int b200_powm(b200_ctx *ctx, const b200_csr *A, const b200_linop *Aop, void *x_dev, const b200_powm_opts *opts,
               b200_result *res, double *lambda_out, double *resnorm_host, int64_t resnorm_cap) {
+  B200_TRY(real_only(A, "b200_powm"));
+  B200_TRY(real_only(Aop ? Aop->dtype : B200_F64, "b200_powm"));
   B200_REQUIRE(ctx && x_dev && opts, "NULL argument");
   B200_REQUIRE((A != nullptr) != (Aop != nullptr), "exactly one of the CSR operator and the callback operator must be given");
   CudaOp op;

@@ -222,6 +222,7 @@ extern "C" {
 int b200_chebyshev_solve(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *b_dev, double lambda_min,
                          double lambda_max, const b200_cg_opts *opts, b200_result *res, double *resnorm_host,
                          int64_t resnorm_cap) {
+  B200_TRY(real_only(A, "b200_chebyshev_solve"));
   B200_REQUIRE(ctx && A && x_dev && b_dev && opts, "NULL argument");
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(is_square(A), "this solver needs a square operator (got %lld x %lld)", (long long)A->m_global,

@@ -13,6 +13,7 @@
 #include <vector>
 
 #include "../../include/b200krylov.h"
+#include "complex.h"
 #include "peer.cuh"
 
 namespace b200 {
@@ -141,8 +142,42 @@ template <>
 struct dtype_of<float> {
   static constexpr int value = B200_F32;
 };
+template <>
+struct dtype_of<cplx<double>> {
+  static constexpr int value = B200_CF64;
+};
+template <>
+struct dtype_of<cplx<float>> {
+  static constexpr int value = B200_CF32;
+};
 
-inline size_t dtype_size(int dtype) { return dtype == B200_F64 ? 8 : 4; }
+inline size_t dtype_size(int dtype) {
+  switch (dtype) {
+    case B200_F64: return 8;
+    case B200_CF64: return 16;
+    case B200_CF32: return 8;
+    default: return 4;
+  }
+}
+inline bool is_complex_dtype(int dtype) { return dtype == B200_CF64 || dtype == B200_CF32; }
+inline const char *dtype_name(int dtype) {
+  switch (dtype) {
+    case B200_F64: return "Float64";
+    case B200_F32: return "Float32";
+    case B200_CF64: return "ComplexF64";
+    case B200_CF32: return "ComplexF32";
+    default: return "an unknown element type";
+  }
+}
+// Entry points without a complex form call this before they touch any data: B200_ERR_UNSUPPORTED for a complex element
+// type (the many "Float64, otherwise Float32" dispatches behind them would read complex data as Float32).
+inline int real_only(int dtype, const char *entry) {
+  if (!is_complex_dtype(dtype)) return B200_OK;
+  set_error("%s: %s is not supported; complex element types are supported by b200_spmv, the BLAS-1 calls, cg! and "
+            "gmres! on single-GPU contexts",
+            entry, dtype_name(dtype));
+  return B200_ERR_UNSUPPORTED;
+}
 
 // ---------------------------------------------------------------- device helpers
 #ifdef __CUDACC__
@@ -231,6 +266,21 @@ __device__ __forceinline__ int ld_stream<int>(const int *p, uint64_t pol) {
   int r;
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.s32 %0, [%1], %2;" : "=r"(r) : "l"(p), "l"(pol));
   return r;
+}
+// complex values: one 16-byte (ComplexF64) / 8-byte (ComplexF32) vector load; p must be aligned to 2 sizeof(R)
+template <>
+__device__ __forceinline__ cplx<double> ld_stream<cplx<double>>(const cplx<double> *p, uint64_t pol) {
+  double re, im;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;"
+               : "=d"(re), "=d"(im) : "l"(p), "l"(pol));
+  return cplx<double>(re, im);
+}
+template <>
+__device__ __forceinline__ cplx<float> ld_stream<cplx<float>>(const cplx<float> *p, uint64_t pol) {
+  float re, im;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;"
+               : "=f"(re), "=f"(im) : "l"(p), "l"(pol));
+  return cplx<float>(re, im);
 }
 
 // Programmatic dependent launch (PDL): consecutive kernels of an iteration are chained so that the blocks of kernel k+1 are

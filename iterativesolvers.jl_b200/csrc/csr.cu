@@ -429,9 +429,10 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
   B200_CUDA(cudaStreamSynchronize(ctx->stream));
   A->max_row_nnz = ctx->h_flags[0];
   A->avg_row_nnz = A->m_local ? (double)A->nnz / (double)A->m_local : 0.0;
-  // TMA-streamed kernel (spmv_stream.cuh): smallest lanes-per-row whose 512/LPR-row tiles hold <= 4096 nonzeros
+  // TMA-streamed kernel (spmv_stream.cuh): smallest lanes-per-row whose 512/LPR-row tiles hold <= 4096 nonzeros.
+  // Complex operators always take the sub-warp form: a ComplexF64 stage would not fit (DESIGN.md, complex element types)
   A->stream_lpr = 0;
-  if (A->m_local > 0) {
+  if (A->m_local > 0 && !is_complex_dtype(A->dtype)) {
     for (int l = 0; l < 6; ++l) {
       B200_CUDA(cudaMemsetAsync(d_max + 1 + l, 0, sizeof(int), ctx->stream));
       k_tile_max<<<grid_for(ctx, (A->m_local + 15) / 16), 256, 0, ctx->stream>>>(A->rowptr, A->m_local, 512 >> l, d_max + 1 + l);
@@ -448,7 +449,7 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
   // band description (csr.cuh): single GPU, and only worth a pass when no row has more than 8 nonzeros and the CSR
   // stream runs with one lane per row
   A->band_ok = false;
-  if (ctx->world == 1 && A->stream_lpr == 1 && A->max_row_nnz <= 8) {
+  if (ctx->world == 1 && A->stream_lpr == 1 && A->max_row_nnz <= 8) {   // never for complex operators (stream_lpr == 0)
     const int64_t ntiles = (A->m_local + kBandTileRows - 1) / kBandTileRows;
     B200_CUDA(cudaMalloc(&A->band_hdr, sizeof(b200_band_tile) * ntiles));
     B200_CUDA(cudaMalloc(&A->band_mask, (size_t)kBandTileRows * ntiles));
@@ -637,7 +638,7 @@ extern "C" {
 int b200_csr_from_csc(b200_ctx *ctx, int64_t m, int64_t n, const void *colptr, const void *rowval, const void *nzval,
                       int idx_bytes, int dtype, int base, b200_csr **out) {
   B200_REQUIRE(ctx && out && colptr && (idx_bytes == 4 || idx_bytes == 8), "bad arguments");
-  B200_REQUIRE(dtype == B200_F64 || dtype == B200_F32, "bad dtype");
+  B200_REQUIRE(dtype == B200_F64 || dtype == B200_F32 || dtype == B200_CF64 || dtype == B200_CF32, "bad dtype");
   B200_REQUIRE(ctx->world == 1, "b200_csr_from_csc is single-GPU; use b200_csr_from_csr_slab on multi-GPU contexts");
   B200_REQUIRE(m >= 0 && n >= 0 && m < INT32_MAX && n < INT32_MAX, "dimensions must fit int32");
   // rectangular operators are accepted (lsqr!/lsmr!); the square-system solvers check is_square(A) themselves
@@ -651,7 +652,15 @@ int b200_csr_from_csc(b200_ctx *ctx, int64_t m, int64_t n, const void *colptr, c
   const int64_t nnz = (idx_bytes == 8 ? (int64_t)((const int64_t *)colptr)[n] : (int64_t)((const int32_t *)colptr)[n]) - base;
   const cudaMemcpyKind h2d = cudaMemcpyHostToDevice;
   int s;
-  if (idx_bytes == 8) {
+  if (is_complex_dtype(dtype)) {
+    // the same upload / sort / gather pipeline with a 16-byte (ComplexF64) or 8-byte (ComplexF32) value type
+    if (idx_bytes == 8)
+      s = dtype == B200_CF64 ? csr_from_csc_impl<int64_t, cplx<double>, cplx<double>>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const cplx<double> *)nzval, base, nnz, h2d, A)
+                             : csr_from_csc_impl<int64_t, cplx<float>, cplx<float>>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const cplx<float> *)nzval, base, nnz, h2d, A);
+    else
+      s = dtype == B200_CF64 ? csr_from_csc_impl<int32_t, cplx<double>, cplx<double>>(ctx, m, n, (const int32_t *)colptr, (const int32_t *)rowval, (const cplx<double> *)nzval, base, nnz, h2d, A)
+                             : csr_from_csc_impl<int32_t, cplx<float>, cplx<float>>(ctx, m, n, (const int32_t *)colptr, (const int32_t *)rowval, (const cplx<float> *)nzval, base, nnz, h2d, A);
+  } else if (idx_bytes == 8) {
     s = dtype == B200_F64 ? csr_from_csc_impl<int64_t, double, double>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const double *)nzval, base, nnz, h2d, A)
                           : csr_from_csc_impl<int64_t, float, float>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const float *)nzval, base, nnz, h2d, A);
   } else {
@@ -671,6 +680,7 @@ int b200_csr_from_csc(b200_ctx *ctx, int64_t m, int64_t n, const void *colptr, c
  * lsmr src/lsmr.jl:117): the device CSR arrays of A are the CSC arrays of A', so the CSC->CSR conversion above builds
  * the CSR of A' without leaving the GPU.  Real element types: adjoint == transpose. */
 int b200_csr_transpose(b200_ctx *ctx, const b200_csr *A, b200_csr **out) {
+  B200_TRY(real_only(A, "b200_csr_transpose"));
   B200_REQUIRE(ctx && A && out, "NULL argument");
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(ctx->world == 1, "b200_csr_transpose is single-GPU; on multi-GPU contexts build the adjoint from its own "
@@ -700,6 +710,7 @@ int b200_csr_transpose(b200_ctx *ctx, const b200_csr *A, b200_csr **out) {
 int b200_csr_from_csr_slab(b200_ctx *ctx, int64_t n_global, int64_t row_begin, int64_t m_local, const void *rowptr,
                            const void *colind, const void *vals, int idx_bytes, int dtype, int base,
                            const b200_halo_plan *plan, b200_csr **out) {
+  B200_TRY(real_only(dtype, "b200_csr_from_csr_slab"));
   B200_REQUIRE(out && rowptr && (idx_bytes == 4 || idx_bytes == 8), "bad arguments");
   B200_REQUIRE(dtype == B200_F64 || dtype == B200_F32, "bad dtype");
   B200_TRY(check_dist_args(ctx, n_global, row_begin, m_local, plan));
@@ -780,6 +791,7 @@ int b200_csr_from_csr_slab(b200_ctx *ctx, int64_t n_global, int64_t row_begin, i
 
 int b200_csr_laplacian(b200_ctx *ctx, int64_t N, int dims, int dtype, int64_t row_begin, int64_t m_local,
                        const b200_halo_plan *plan, b200_csr **out) {
+  B200_TRY(real_only(dtype, "b200_csr_laplacian"));
   B200_REQUIRE(out && N >= 1 && dims >= 1 && dims <= 6, "bad arguments");
   B200_REQUIRE(dtype == B200_F64 || dtype == B200_F32, "bad dtype");
   LapGeom g;
@@ -904,7 +916,11 @@ int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes)
 int b200_csr_diag(b200_ctx *ctx, const b200_csr *A, void *diag_dev) {
   B200_REQUIRE(ctx && A && diag_dev, "NULL argument");
   if (A->m_local == 0) return B200_OK;
-  if (A->dtype == B200_F64)
+  if (A->dtype == B200_CF64)
+    k_diag<cplx<double>><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const cplx<double> *)A->vals, A->m_local, (cplx<double> *)diag_dev);
+  else if (A->dtype == B200_CF32)
+    k_diag<cplx<float>><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const cplx<float> *)A->vals, A->m_local, (cplx<float> *)diag_dev);
+  else if (A->dtype == B200_F64)
     k_diag<double><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const double *)A->vals, A->m_local, (double *)diag_dev);
   else
     k_diag<float><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const float *)A->vals, A->m_local, (float *)diag_dev);

@@ -75,6 +75,8 @@ int halo_exchange(b200_ctx *ctx, const b200_csr *A, const void *x_dev);
 // (skipped on the device when *done_flag != 0); consumers wait with peer_wait_halo(.., A->recv_mask, seq)
 int halo_push(b200_ctx *ctx, const b200_csr *A, const void *x_dev, unsigned long long seq, const int *done_flag);
 inline bool is_square(const b200_csr *A) { return A->m_global == A->n_global; }
+// real_only (common.cuh) for an operator argument (NULL is left to the entry point's own argument check)
+inline int real_only(const b200_csr *A, const char *entry) { return A ? real_only(A->dtype, entry) : B200_OK; }
 inline bool use_peer(const b200_ctx *ctx, const b200_csr *A) {
   return ctx->world > 1 && ctx->peer_ok && A->peer_halo && ctx->opt_comm != 1;
 }

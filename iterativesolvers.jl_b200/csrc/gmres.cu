@@ -890,6 +890,7 @@ extern "C" {
 
 int b200_orthogonalize_and_normalize(b200_ctx *ctx, int64_t n_local, const void *V_dev, int64_t ldv, int k, void *w_dev,
                                      double *h_host, int method, int dtype, double *nrm) {
+  B200_TRY(real_only(dtype, "b200_orthogonalize_and_normalize"));
   B200_REQUIRE(ctx && w_dev && nrm && (k == 0 || (V_dev && h_host)), "NULL argument");
   B200_REQUIRE(ldv >= n_local && n_local >= 0, "bad leading dimension");
   B200_REQUIRE(method == B200_ORTH_MGS || method == B200_ORTH_CGS || method == B200_ORTH_DGKS, "bad orth_meth");
@@ -912,7 +913,8 @@ int b200_gmres_solve(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(is_square(A), "this solver needs a square operator (got %lld x %lld)", (long long)A->m_global,
                (long long)A->n_global);
-  if (opts->Pl.kind == B200_PREC_CALLBACK || opts->Pr.kind == B200_PREC_CALLBACK)     // ldiv! callbacks: the general engine
+  // ldiv! callbacks, or a complex operator (the engine below is real-only): the general engine
+  if (opts->Pl.kind == B200_PREC_CALLBACK || opts->Pr.kind == B200_PREC_CALLBACK || is_complex_dtype(A->dtype))
     return gmres_general(ctx, CudaOp{A, nullptr}, A->dtype, A->m_local, A->n_global, x_dev, b_dev, opts, res, resnorm_host,
                          resnorm_cap);
   B200_REQUIRE(opts->Pl.kind == B200_PREC_IDENTITY || (opts->Pl.kind == B200_PREC_JACOBI && opts->Pl.diag),

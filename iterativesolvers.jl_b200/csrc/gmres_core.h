@@ -16,9 +16,16 @@
 //   scale        w *= inv(nrm)                                                                                   :36
 //   step         H[:, k] ; nullvec recurrence ; residual ; at the end of a cycle the Givens LS solve            :224-233, :262-271
 //   update       x += V[:, 1:k-1] y  (through Pr when given)                                                     :273-283
+//
+// Complex element types (T = cplx<R>): the scalar block is GmScalC, where H, h, corr, nullvec and rhs are complex (fp64
+// for ComplexF32 too); every dot is Julia's dot(x, y) = sum conj(x_i) y_i and takes two of a pass's sums, so a CGS / DGKS
+// dot pass covers 8 basis columns instead of 16; norms and the DGKS projection sizes use abs2; the least-squares solve
+// uses the complex givensAlgorithm with the -conj(s) rotations of src/hessenberg.jl:32,38.  The real instantiations are
+// the code they were before complex types existed (if constexpr, overloads on the scalar block).
 #pragma once
 #include <memory>
 
+#include "complex.h"
 #include "pass_core.h"
 
 namespace b200 {
@@ -43,10 +50,36 @@ struct GmScal {
   int k, restart, m, flags, first, reorth, pad0, pad1;
 };
 
-B200_HD bool gm_done(const GmScal *q, long long it) { return it >= q->maxiter || q->current <= q->tol; }   // done :55
+struct GmScalC {                      // GmScal of the complex element types
+  cplx<double> H[kGmLdh * kGmMaxRestart];
+  cplx<double> nullvec[kGmLdh];
+  cplx<double> rhs[kGmLdh];
+  cplx<double> h[kGmMaxRestart], corr[kGmMaxRestart];
+  double accumulator, current, beta_res, beta, tol, abstol, reltol;
+  double nrm2, nrm, proj;
+  double sum[kPassMaxRed];
+  double *hist;
+  long long hist_cap, n_hist, iteration, maxiter;
+  int k, restart, m, flags, first, reorth, pad0, pad1;
+};
+template <typename T>
+struct gm_scal {
+  typedef GmScal type;
+};
+template <typename R>
+struct gm_scal<cplx<R>> {
+  typedef GmScalC type;
+};
+// basis columns per dot pass: one sum per column, two (re, im) for complex T
+template <typename T>
+constexpr int gm_dot_block() { return is_cplx<T>::value ? kGmBlock / 2 : kGmBlock; }
+
+template <typename Q>
+B200_HD bool gm_done(const Q *q, long long it) { return it >= q->maxiter || q->current <= q->tol; }   // done :55
 
 // after the norm of the (preconditioned) residual is known: init! :252 and what follows it at :126-133 / :96-99
-B200_HD void gm_set_beta(GmScal *q, double sumsq) {
+template <typename Q>
+B200_HD void gm_set_beta(Q *q, double sumsq) {
   const double beta = sqrt(sumsq);
   q->beta = beta;                               // g.beta :133 / :96
   q->accumulator = 1.0;                         // init_residual! :257-260
@@ -66,7 +99,7 @@ struct GmResidual {
   static constexpr int NRED = 1;
   const T *b, *ax, *diag;      // ax: A*x or nullptr (initially_zero); diag: Jacobi Pl or nullptr
   T *out;
-  GmScal *s;
+  typename gm_scal<T>::type *s;
   int is_beta;                 // the norm of this pass is beta (no callback preconditioner follows)
   B200_HD bool skip() const { return false; }
   B200_HD void load() {}
@@ -75,7 +108,8 @@ struct GmResidual {
     if (ax) r = r - ax[i];                       // first_col .-= Ax :246
     if (diag) r = r / diag[i];                   // ldiv!(Pl, first_col) :249
     out[i] = r;
-    acc[0] += (double)r * (double)r;
+    if constexpr (is_cplx<T>::value) acc[0] += (double)r.re * (double)r.re + (double)r.im * (double)r.im;
+    else acc[0] += (double)r * (double)r;
   }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
@@ -87,10 +121,13 @@ template <typename T>
 struct GmNorm {                // norm(first_col) after a callback preconditioner :252
   static constexpr int NRED = 1;
   const T *v;
-  GmScal *s;
+  typename gm_scal<T>::type *s;
   B200_HD bool skip() const { return false; }
   B200_HD void load() {}
-  B200_HD void elem(int64_t i, double *acc) const { acc[0] += (double)v[i] * (double)v[i]; }
+  B200_HD void elem(int64_t i, double *acc) const {
+    if constexpr (is_cplx<T>::value) acc[0] += (double)v[i].re * (double)v[i].re + (double)v[i].im * (double)v[i].im;
+    else acc[0] += (double)v[i] * (double)v[i];
+  }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const { gm_set_beta(s, tot[0]); }
 };
@@ -139,10 +176,10 @@ struct GmAdd {
 // coefficient and the next dot product share the read of w.
 template <typename T>
 struct GmMgs {
-  static constexpr int NRED = 1;
+  static constexpr int NRED = is_cplx<T>::value ? 2 : 1;
   const T *vprev, *vi;         // vprev: column whose projection is removed now (nullptr on the first pass);
   T *w;                        // vi: column of the next dot (nullptr on the last pass: ||w||^2 instead)
-  GmScal *s;
+  typename gm_scal<T>::type *s;
   int iprev, icur;
   T hprev;
   B200_HD bool skip() const { return false; }
@@ -153,13 +190,24 @@ struct GmMgs {
       wi = wi - hprev * vprev[i];                // w .-= h[i] .* column :72
       w[i] = wi;
     }
-    acc[0] += vi ? (double)vi[i] * (double)wi    // h[i] = dot(column, w) :71
-                 : (double)wi * (double)wi;      // nrm = norm(w) :75
+    if constexpr (is_cplx<T>::value) {
+      if (vi) {                                  // h[i] = dot(column, w) = sum conj(column) w :71
+        const T v = vi[i];
+        acc[0] += (double)v.re * (double)wi.re + (double)v.im * (double)wi.im;
+        acc[1] += (double)v.re * (double)wi.im - (double)v.im * (double)wi.re;
+      } else {
+        acc[0] += (double)wi.re * (double)wi.re + (double)wi.im * (double)wi.im;   // nrm = norm(w) :75
+      }
+    } else {
+      acc[0] += vi ? (double)vi[i] * (double)wi    // h[i] = dot(column, w) :71
+                   : (double)wi * (double)wi;      // nrm = norm(w) :75
+    }
   }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
     if (vi) {
-      s->h[icur] = tot[0];
+      if constexpr (is_cplx<T>::value) s->h[icur] = cplx<double>(tot[0], tot[1]);
+      else s->h[icur] = tot[0];
     } else {
       s->nrm2 = tot[0];
       s->nrm = sqrt(tot[0]);
@@ -173,21 +221,36 @@ struct GmDots {
   static constexpr int NRED = kGmBlock;
   const T *V;                  // first column of the chunk
   int64_t ld;
-  int cnt, j0, to_corr;
+  int cnt, j0, to_corr;         // cnt <= gm_dot_block<T>()
   const T *w;
-  GmScal *s;
+  typename gm_scal<T>::type *s;
   B200_HD bool skip() const { return false; }
   B200_HD void load() {}
   B200_HD void elem(int64_t i, double *acc) const {
-    const double wv = (double)w[i];
-    B200_UNROLL
-    for (int j = 0; j < kGmBlock; ++j)
-      if (j < cnt) acc[j] += (double)V[i + j * ld] * wv;
+    if constexpr (is_cplx<T>::value) {           // sum conj(V[:, j]) w: (re, im) in acc[2j], acc[2j+1]
+      const T wv = w[i];
+      B200_UNROLL
+      for (int j = 0; j < kGmBlock / 2; ++j)
+        if (j < cnt) {
+          const T v = V[i + j * ld];
+          acc[2 * j] += (double)v.re * (double)wv.re + (double)v.im * (double)wv.im;
+          acc[2 * j + 1] += (double)v.re * (double)wv.im - (double)v.im * (double)wv.re;
+        }
+    } else {
+      const double wv = (double)w[i];
+      B200_UNROLL
+      for (int j = 0; j < kGmBlock; ++j)
+        if (j < cnt) acc[j] += (double)V[i + j * ld] * wv;
+    }
   }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
-    double *dst = to_corr ? s->corr : s->h;
-    for (int j = 0; j < cnt; ++j) dst[j0 + j] = tot[j];
+    auto *dst = to_corr ? s->corr : s->h;
+    if constexpr (is_cplx<T>::value) {
+      for (int j = 0; j < cnt; ++j) dst[j0 + j] = cplx<double>(tot[2 * j], tot[2 * j + 1]);
+    } else {
+      for (int j = 0; j < cnt; ++j) dst[j0 + j] = tot[j];
+    }
   }
 };
 
@@ -202,11 +265,11 @@ struct GmUpdate {
   int cnt, j0, which;
   double sign;
   T *w;
-  GmScal *s;
+  typename gm_scal<T>::type *s;
   T c[kGmBlock];
   B200_HD bool skip() const { return false; }
   B200_HD void load() {
-    const double *src = which == GM_COEF_H ? s->h : (which == GM_COEF_CORR ? s->corr : s->rhs);
+    const auto *src = which == GM_COEF_H ? s->h : (which == GM_COEF_CORR ? s->corr : s->rhs);
     B200_UNROLL
     for (int j = 0; j < kGmBlock; ++j) c[j] = j < cnt ? (T)(sign * src[j0 + j]) : (T)0;
   }
@@ -217,7 +280,11 @@ struct GmUpdate {
       if (j < cnt) t = t + V[i + j * ld] * c[j];
     const T wi = w[i] + t;
     w[i] = wi;
-    if (NORM) acc[0] += (double)wi * (double)wi;
+    if constexpr (is_cplx<T>::value) {
+      if (NORM) acc[0] += (double)wi.re * (double)wi.re + (double)wi.im * (double)wi.im;
+    } else {
+      if (NORM) acc[0] += (double)wi * (double)wi;
+    }
   }
   B200_HD double *sums() const { return s->sum; }
   B200_HD void finish(const double *tot) const {
@@ -300,6 +367,95 @@ B200_HD void gm_step(GmScal *q) {
   q->flags = flags;
 }
 
+// ---- complex forms of the scalar sections above (GmScalC)
+B200_HD void gm_dgks_first(GmScalC *q) {
+  double p = 0.0;
+  for (int j = 0; j < q->k; ++j) p += abs2(q->h[j]);
+  q->proj = sqrt(p);                                             // projection_size = norm(h) :22
+  q->reorth = q->nrm < (1.0 / sqrt(2.0)) * q->proj;              // :26
+}
+B200_HD void gm_dgks_next(GmScalC *q) {
+  double p = 0.0;
+  for (int j = 0; j < q->k; ++j) {
+    p += abs2(q->corr[j]);
+    q->h[j] += q->corr[j];                                       // h .+= correction :31
+  }
+  q->proj = sqrt(p);                                             // :28
+  q->reorth = q->nrm < (1.0 / sqrt(2.0)) * q->proj;
+}
+// LinearAlgebra.givensAlgorithm(f, g) for complex arguments -> (c real, s, r) with [c s; -conj(s) c][f; g] = [r; 0]
+// (c = |f| / d, s = (f / |f|) conj(g) / d, r = (f / |f|) d, d = hypot(|f|, |g|)).  For real f, g it differs from
+// givens_real only in sign: (-c, -s, -r) when f < 0 and |f| <= |g| (and s = sign(g) when f == 0), which negates both
+// rotated rows -- the back-substitution cancels it exactly.
+B200_HD void givens_cplx(cplx<double> f, cplx<double> g, double &c, cplx<double> &s, cplx<double> &r) {
+  if (g.re == 0.0 && g.im == 0.0) { c = 1.0; s = cplx<double>(0.0); r = f; return; }
+  if (f.re == 0.0 && f.im == 0.0) {
+    const double ag = hypot(g.re, g.im);
+    c = 0.0; s = cplx<double>(g.re / ag, -g.im / ag); r = cplx<double>(ag); return;
+  }
+  const double f1 = hypot(f.re, f.im), g1 = hypot(g.re, g.im), d = hypot(f1, g1);
+  const cplx<double> ph(f.re / f1, f.im / f1), t = ph * conj(g);
+  c = f1 / d;
+  s = cplx<double>(t.re / d, t.im / d);
+  r = cplx<double>(ph.re * d, ph.im * d);
+}
+// ldiv!(FastHessenberg(H[1:m+1, 1:m]), rhs[1:m+1]) of src/hessenberg.jl:15-46, column-major H with leading dimension ldh
+B200_HD void gm_hessenberg_solve_c(cplx<double> *H, int ldh, int m, cplx<double> *rhs) {
+  for (int i = 0; i < m; ++i) {                                  // :24
+    double c;
+    cplx<double> s, r;
+    givens_cplx(H[i + i * ldh], H[i + 1 + i * ldh], c, s, r);
+    H[i + i * ldh] = c * H[i + i * ldh] + s * H[i + 1 + i * ldh];   // :28
+    for (int j = i + 1; j < m; ++j) {                            // :31-35
+      const cplx<double> a = H[i + j * ldh], b = H[i + 1 + j * ldh];
+      H[i + j * ldh] = c * a + s * b;
+      H[i + 1 + j * ldh] = -conj(s) * a + c * b;
+    }
+    const cplx<double> a = rhs[i], b = rhs[i + 1];               // :38-40
+    rhs[i] = c * a + s * b;
+    rhs[i + 1] = -conj(s) * a + c * b;
+  }
+  for (int i = m - 1; i >= 0; --i) {                             // UpperTriangular solve :44-45
+    cplx<double> acc = rhs[i];
+    for (int j = i + 1; j < m; ++j) acc -= H[i + j * ldh] * rhs[j];
+    rhs[i] = acc / H[i + i * ldh];
+  }
+}
+B200_HD void gm_step(GmScalC *q) {
+  const int k = q->k, col = k - 1;
+  cplx<double> *Hc = q->H + (size_t)col * kGmLdh;
+  for (int j = 0; j < k; ++j) Hc[j] = q->h[j];                   // H[1:k, k] :68-73
+  Hc[k] = cplx<double>(q->nrm);                                  // H[k+1, k] = orthogonalize_and_normalize!(...)
+  if (q->nrm == 0.0) {                                           // update_residual! :224-233
+    q->current = 0.0;
+  } else {
+    cplx<double> d(0.0);
+    for (int j = 0; j < k; ++j) d += conj(q->nullvec[j]) * Hc[j];   // dot(nullvec[1:k], H[1:k, k])
+    q->nullvec[k] = -conj(d / Hc[k]);                            // :229
+    q->accumulator += abs2(q->nullvec[k]);                       // :230
+    q->current = q->beta_res / sqrt(q->accumulator);
+  }
+  int flags = 0;
+  const int k1 = k + 1;                                          // :78
+  q->k = k1;
+  if (k1 == q->restart + 1 || gm_done(q, q->iteration + 1)) {    // :82
+    const int m = k1 - 1;                                        // solve_least_squares! :262-271
+    for (int i = 0; i <= m; ++i) q->rhs[i] = cplx<double>(0.0);
+    q->rhs[0] = cplx<double>(q->beta);                           // :265
+    gm_hessenberg_solve_c(q->H, kGmLdh, m, q->rhs);
+    q->m = m;
+    q->k = 1;                                                    // :90
+    flags |= GM_FIN;
+    if (!gm_done(q, q->iteration)) flags |= GM_REINIT;           // :93 (sic: the old iteration count)
+  }
+  q->iteration += 1;
+  if (q->hist && q->n_hist < q->hist_cap) q->hist[q->n_hist] = q->current;   // push!(history, :resnorm, ...) :211
+  q->n_hist += 1;
+  if (gm_done(q, q->iteration)) flags |= GM_DONE;                // :59
+  if (!(q->current == q->current)) flags |= GM_DONE | GM_BREAKDOWN;
+  q->flags = flags;
+}
+
 struct GmresOutcome {
   int64_t iters, mvps, n_hist;
   double residual, tol;
@@ -312,14 +468,14 @@ template <typename T>
 struct GmresLayout {
   T *V, *t1, *t2;
   int64_t ld;
-  GmScal *s;
+  typename gm_scal<T>::type *s;
   double *hist;
   int64_t hist_cap;
 };
 inline size_t gm_vec_bytes(size_t elem, int64_t n) { return ((elem * (size_t)(n > 0 ? n : 1)) + 255) / 256 * 256; }
 template <typename T>
 size_t gmres_ws_bytes(int64_t n, int restart, int64_t hist_cap) {
-  return gm_vec_bytes(sizeof(T), n) * (size_t)(restart + 3) + (sizeof(GmScal) + 255) / 256 * 256 +
+  return gm_vec_bytes(sizeof(T), n) * (size_t)(restart + 3) + (sizeof(typename gm_scal<T>::type) + 255) / 256 * 256 +
          ((sizeof(double) * (size_t)(hist_cap > 0 ? hist_cap : 1)) + 255) / 256 * 256;
 }
 template <typename T>
@@ -331,7 +487,8 @@ GmresLayout<T> gmres_layout(void *ws, int64_t n, int restart, int64_t hist_cap) 
   L.t1 = (T *)p; p += vb;
   L.t2 = (T *)p; p += vb;
   L.ld = (int64_t)(vb / sizeof(T));
-  L.s = (GmScal *)p; p += (sizeof(GmScal) + 255) / 256 * 256;
+  typedef typename gm_scal<T>::type Scal;
+  L.s = (Scal *)p; p += (sizeof(Scal) + 255) / 256 * 256;
   L.hist = hist_cap > 0 ? (double *)p : nullptr;
   L.hist_cap = hist_cap > 0 ? hist_cap : 0;
   return L;
@@ -351,7 +508,7 @@ int gmres_init_residual(B &be, const GmresOps<T, B> &op, const GmresLayout<T> &L
                         bool zero) {
   int s2;
   T *v0 = L.V, *t1 = L.t1, *t2 = L.t2;
-  GmScal *s = L.s;
+  typename gm_scal<T>::type *s = L.s;
   if (!zero && (s2 = be.apply(op.A, x, t1))) return s2;                     // mul!(Ax, A, x) :245
   if (op.Pl) {
     if ((s2 = be.pass(GmResidual<T>{b, zero ? nullptr : t1, nullptr, t2, s, 0}, n))) return s2;
@@ -371,6 +528,7 @@ int gmres_setup(B &be, const GmresOps<T, B> &op, const GmresLayout<T> &L, int64_
   if (restart < 1 || restart > kGmMaxRestart) return -1;                    // B200_ERR_INVALID (checked by the callers)
   int st;
   {
+    typedef typename gm_scal<T>::type GmScal;
     std::unique_ptr<GmScal> h(new GmScal);
     memset(h.get(), 0, sizeof(GmScal));
     for (int i = 0; i < kGmLdh; ++i) h->nullvec[i] = 1.0;                   // ones(T, order + 1) :27
@@ -396,6 +554,7 @@ int gmres_advance(B &be, const GmresOps<T, B> &op, const GmresLayout<T> &L, int6
                   int64_t kmax, int64_t *mv_products) {
   T *V = L.V, *t1 = L.t1, *t2 = L.t2;
   const int64_t ld = L.ld;
+  typedef typename gm_scal<T>::type GmScal;
   GmScal *s = L.s;
   const typename B::Op *A = op.A, *Pl = op.Pl, *Pr = op.Pr;
   const T *pl_diag = op.pl_diag, *pr_diag = op.pr_diag;
@@ -432,8 +591,9 @@ int gmres_advance(B &be, const GmresOps<T, B> &op, const GmresLayout<T> &L, int6
           return s2;
     } else {
       auto dots = [&](int to_corr) -> int {
-        for (int j0 = 0; j0 < k; j0 += kGmBlock) {
-          const int cnt = k - j0 < kGmBlock ? k - j0 : kGmBlock;
+        constexpr int DB = gm_dot_block<T>();
+        for (int j0 = 0; j0 < k; j0 += DB) {
+          const int cnt = k - j0 < DB ? k - j0 : DB;
           const int s3 = be.pass(GmDots<T>{col(j0), ld, cnt, j0, to_corr, w, s}, n);
           if (s3) return s3;
         }
@@ -518,6 +678,7 @@ int gmres_advance(B &be, const GmresOps<T, B> &op, const GmresLayout<T> &L, int6
 template <typename T, typename B>
 int gmres_collect(B &be, const GmresLayout<T> &L, int64_t mv_products, double *hist_host, GmresOutcome *out) {
   int st;
+  typedef typename gm_scal<T>::type GmScal;
   std::unique_ptr<GmScal> h(new GmScal);
   if ((st = be.to_host(h.get(), L.s, sizeof(GmScal)))) return st;
   out->iters = h->iteration;
@@ -531,8 +692,8 @@ int gmres_collect(B &be, const GmresLayout<T> &L, int64_t mv_products, double *h
   if (hist_host && out->n_hist > 0 && (st = be.to_host(hist_host, L.hist, sizeof(double) * (size_t)out->n_hist))) return st;
   return 0;
 }
-template <typename B>
-int gmres_reset_window(B &be, GmScal *s) {
+template <typename B, typename Q>
+int gmres_reset_window(B &be, Q *s) {
   const long long zero = 0;
   return be.to_device(&s->n_hist, &zero, sizeof(zero));
 }

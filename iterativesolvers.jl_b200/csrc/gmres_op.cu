@@ -19,7 +19,7 @@ static int side(const b200_precond &P, const char *what, int dtype, int64_t n, c
     return B200_OK;
   }
   *fn = (const b200_linop *)P.diag;
-  B200_TRY(check_linop(*fn, what));
+  B200_TRY(check_linop_complex(*fn, what));
   B200_REQUIRE((*fn)->dtype == dtype && (*fn)->m_local == n && (*fn)->n_local == n,
                "%s must act on vectors of the operator's local length", what);
   return B200_OK;
@@ -29,6 +29,10 @@ int gmres_general(b200_ctx *ctx, const CudaOp &A, int dtype, int64_t n, int64_t 
                   const b200_gmres_opts *opts, b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
   const b200_linop *plf, *prf;
   const void *pld, *prd;
+  if (is_complex_dtype(dtype) && ctx->world > 1) {
+    set_error("gmres!: %s operators are single-GPU in this version", dtype_name(dtype));
+    return B200_ERR_UNSUPPORTED;
+  }
   B200_TRY(side(opts->Pl, "Pl", dtype, n, &plf, &pld));
   B200_TRY(side(opts->Pr, "Pr", dtype, n, &prf, &prd));
   const int restart = opts->restart > 0 ? opts->restart : (int)std::min<int64_t>(20, n_global);   // src/gmres.jl:188
@@ -40,7 +44,19 @@ int gmres_general(b200_ctx *ctx, const CudaOp &A, int dtype, int64_t n, int64_t 
   CudaOp pl{nullptr, plf}, pr{nullptr, prf};
   GmresOutcome o;
   memset(&o, 0, sizeof(o));
-  const int st =
+  int st;
+  if (dtype == B200_CF64)
+    st = gmres_run<cplx<double>>(be, &A, plf ? &pl : nullptr, prf ? &pr : nullptr, (const cplx<double> *)pld,
+                                 (const cplx<double> *)prd, n, n_global, (cplx<double> *)x_dev, (const cplx<double> *)b_dev,
+                                 opts->abstol, opts->reltol, restart, opts->maxiter, opts->initially_zero, opts->orth_meth,
+                                 resnorm_cap, resnorm_host, &o);
+  else if (dtype == B200_CF32)
+    st = gmres_run<cplx<float>>(be, &A, plf ? &pl : nullptr, prf ? &pr : nullptr, (const cplx<float> *)pld,
+                                (const cplx<float> *)prd, n, n_global, (cplx<float> *)x_dev, (const cplx<float> *)b_dev,
+                                opts->abstol, opts->reltol, restart, opts->maxiter, opts->initially_zero, opts->orth_meth,
+                                resnorm_cap, resnorm_host, &o);
+  else
+    st =
       dtype == B200_F64
           ? gmres_run<double>(be, &A, plf ? &pl : nullptr, prf ? &pr : nullptr, (const double *)pld, (const double *)prd, n,
                               n_global, (double *)x_dev, (const double *)b_dev, opts->abstol, opts->reltol, restart,
@@ -68,7 +84,7 @@ extern "C" {
 int b200_gmres_solve_op(b200_ctx *ctx, const b200_linop *A, void *x_dev, const void *b_dev, const b200_gmres_opts *opts,
                         b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
   B200_REQUIRE(ctx && x_dev && b_dev && opts, "NULL argument");
-  B200_TRY(check_linop(A, "A"));
+  B200_TRY(check_linop_complex(A, "A"));
   B200_REQUIRE(A->m_global == A->n_global && A->m_local == A->n_local, "gmres! needs a square operator");
   return gmres_general(ctx, CudaOp{nullptr, A}, A->dtype, A->m_local, A->n_global, x_dev, b_dev, opts, res, resnorm_host,
                        resnorm_cap);

@@ -57,6 +57,7 @@ extern "C" {
 
 int b200_idrs_solve(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *b_dev, const b200_idrs_opts *opts,
                     b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
+  B200_TRY(real_only(A, "b200_idrs_solve"));
   B200_REQUIRE(ctx && A && x_dev && b_dev && opts, "NULL argument");
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(is_square(A), "idrs! needs a square operator (got %lld x %lld)", (long long)A->m_global,
@@ -67,6 +68,7 @@ int b200_idrs_solve(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *b
 
 int b200_idrs_solve_op(b200_ctx *ctx, const b200_linop *A, void *x_dev, const void *b_dev, const b200_idrs_opts *opts,
                        b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_idrs_solve_op"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts, "NULL argument");
   B200_TRY(check_linop(A, "A"));
   B200_REQUIRE(A->m_global == A->n_global && A->m_local == A->n_local, "idrs! needs a square operator");

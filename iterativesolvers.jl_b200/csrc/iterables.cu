@@ -169,6 +169,8 @@ extern "C" {
 
 int b200_gmres_iter_create(b200_ctx *ctx, const b200_csr *A, const b200_linop *Aop, void *x_dev, const void *b_dev,
                            const b200_gmres_opts *opts, b200_iter **out) {
+  B200_TRY(real_only(A, "b200_gmres_iter_create"));
+  B200_TRY(real_only(Aop ? Aop->dtype : B200_F64, "b200_gmres_iter_create"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts && out, "NULL argument");
   std::unique_ptr<b200_iter> it(new b200_iter());
   it->kind = IT_GMRES;
@@ -207,6 +209,8 @@ int b200_gmres_iter_create(b200_ctx *ctx, const b200_csr *A, const b200_linop *A
 
 int b200_minres_iter_create(b200_ctx *ctx, const b200_csr *A, const b200_linop *Aop, void *x_dev, const void *b_dev,
                             const b200_minres_opts *opts, b200_iter **out) {
+  B200_TRY(real_only(A, "b200_minres_iter_create"));
+  B200_TRY(real_only(Aop ? Aop->dtype : B200_F64, "b200_minres_iter_create"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts && out, "NULL argument");
   std::unique_ptr<b200_iter> it(new b200_iter());
   it->kind = IT_MINRES;
@@ -235,6 +239,8 @@ int b200_minres_iter_create(b200_ctx *ctx, const b200_csr *A, const b200_linop *
 
 int b200_bicgstabl_iter_create(b200_ctx *ctx, const b200_csr *A, const b200_linop *Aop, void *x_dev, const void *b_dev,
                                const b200_bicgstabl_opts *opts, b200_iter **out) {
+  B200_TRY(real_only(A, "b200_bicgstabl_iter_create"));
+  B200_TRY(real_only(Aop ? Aop->dtype : B200_F64, "b200_bicgstabl_iter_create"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts && out, "NULL argument");
   B200_REQUIRE(opts->l >= 1 && opts->l <= kBcMaxL, "bicgstabl!: l=%d not in 1..%d", opts->l, kBcMaxL);
   B200_REQUIRE(opts->r_shadow, "r_shadow (device vector) is required: the reference draws rand(T, n) "
@@ -275,6 +281,8 @@ int b200_bicgstabl_iter_create(b200_ctx *ctx, const b200_csr *A, const b200_lino
 // the CSR + Identity / Jacobi form is b200_cg_iter_create (tuned engine, caller-owned state vectors).
 int b200_cg_iter_create_op(b200_ctx *ctx, const b200_csr *A, const b200_linop *Aop, void *x_dev, const void *b_dev,
                            const b200_cg_opts *opts, b200_iter **out) {
+  B200_TRY(real_only(A, "b200_cg_iter_create_op"));
+  B200_TRY(real_only(Aop ? Aop->dtype : B200_F64, "b200_cg_iter_create_op"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts && out, "NULL argument");
   B200_REQUIRE(!opts->fixed_iterations && !opts->variant, "fixed_iterations / variant are not available on this path");
   std::unique_ptr<b200_iter> it(new b200_iter());

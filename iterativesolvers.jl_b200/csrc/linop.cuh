@@ -3,7 +3,8 @@
 #include "pass.cuh"
 
 namespace b200 {
-int check_linop(const b200_linop *A, const char *what);   // qmr.cu
+int check_linop(const b200_linop *A, const char *what);           // qmr.cu; real element types only
+int check_linop_complex(const b200_linop *A, const char *what);   // qmr.cu; also ComplexF64 / ComplexF32 (cg_op, gmres_op)
 // the general (fused-pass) engines behind both the *_solve_op entry points and the b200_csr entry points when one of
 // their preconditioners is a callback
 int gmres_general(b200_ctx *ctx, const CudaOp &A, int dtype, int64_t n, int64_t n_global, void *x_dev, const void *b_dev,

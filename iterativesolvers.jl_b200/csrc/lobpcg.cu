@@ -1366,6 +1366,7 @@ extern "C" {
 
 int b200_lobpcg_solve(b200_ctx *ctx, const b200_csr *A, void *X_dev, int64_t ldx, const b200_lobpcg_opts *opts,
                       b200_lobpcg_result *res, double *lambda_host, double *resnorm_host) {
+  B200_TRY(real_only(A, "b200_lobpcg_solve"));
   B200_REQUIRE(ctx && A && X_dev && opts, "NULL argument");
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(is_square(A), "this solver needs a square operator (got %lld x %lld)", (long long)A->m_global,
@@ -1381,6 +1382,7 @@ int b200_lobpcg_solve(b200_ctx *ctx, const b200_csr *A, void *X_dev, int64_t ldx
 int b200_lobpcg_solve_constrained(b200_ctx *ctx, const b200_csr *A, void *X_dev, int64_t ldx,
                                   const b200_lobpcg_opts *opts, const b200_lobpcg_constraint *C,
                                   b200_lobpcg_result *res, double *lambda_host, double *resnorm_host) {
+  B200_TRY(real_only(A, "b200_lobpcg_solve_constrained"));
   B200_REQUIRE(ctx && A && X_dev && opts, "NULL argument");
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(is_square(A), "this solver needs a square operator (got %lld x %lld)", (long long)A->m_global,

@@ -42,6 +42,7 @@ extern "C" {
 
 int b200_lobpcg_constraint_create(b200_ctx *ctx, int64_t n_local, const void *Y_dev, int64_t ldy, int nc, int capacity,
                                   int dtype, b200_lobpcg_constraint **out) {
+  B200_TRY(real_only(dtype, "b200_lobpcg_constraint_create"));
   B200_REQUIRE(ctx && out && n_local >= 0 && nc >= 0 && (nc == 0 || (Y_dev && ldy >= n_local)), "bad arguments");
   B200_REQUIRE(dtype == B200_F64 || dtype == B200_F32, "bad dtype");
   B200_CUDA(cudaSetDevice(ctx->device));

@@ -34,6 +34,8 @@ int b200_csr_as_linop(const b200_csr *A, b200_linop *out) {
 int b200_lobpcg_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *B, void *X_dev, int64_t ldx,
                          const b200_lobpcg_opts *opts, const b200_lobpcg_constraint *C, b200_lobpcg_result *res,
                          double *lambda_host, double *resnorm_host) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_lobpcg_solve_op"));
+  B200_TRY(real_only(B ? B->dtype : B200_F64, "b200_lobpcg_solve_op"));
   B200_REQUIRE(ctx && X_dev && opts, "NULL argument");
   B200_TRY(check_linop(A, "A"));
   B200_REQUIRE(A->m_global == A->n_global && A->m_local == A->n_local, "lobpcg needs a square operator");
@@ -104,6 +106,8 @@ int b200_lobpcg_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *B
 // the factor is that of Y' BY.
 int b200_lobpcg_constraint_create_b(b200_ctx *ctx, const b200_linop *B, int64_t n_local, const void *Y_dev, int64_t ldy,
                                     int nc, int capacity, int dtype, b200_lobpcg_constraint **out) {
+  B200_TRY(real_only(B ? B->dtype : B200_F64, "b200_lobpcg_constraint_create_b"));
+  B200_TRY(real_only(dtype, "b200_lobpcg_constraint_create_b"));
   B200_REQUIRE(ctx && out && B && nc >= 0 && (nc == 0 || (Y_dev && ldy >= n_local)), "bad arguments");
   B200_TRY(check_linop(B, "B"));
   B200_REQUIRE(B->dtype == dtype && B->m_local == n_local && B->n_local == n_local, "B does not match the constraint");

@@ -99,6 +99,8 @@ extern "C" {
 
 int b200_lsqr_solve(b200_ctx *ctx, const b200_csr *A, const b200_csr *At, void *x_dev, const void *b_dev,
                     const b200_lsq_opts *opts, b200_lsq_result *res, double *hist_host, int64_t hist_cap) {
+  B200_TRY(real_only(A, "b200_lsqr_solve"));
+  B200_TRY(real_only(At, "b200_lsqr_solve"));
   B200_TRY(check_ls_args(ctx, A, At, x_dev, b_dev, opts));
   return lsq_dispatch<false>(ctx, CudaOp{A, nullptr}, CudaOp{At, nullptr}, A->dtype, A->m_local, At->m_local,
                              A->m_global, A->n_global, x_dev, b_dev, opts, res, hist_host, hist_cap);
@@ -106,6 +108,8 @@ int b200_lsqr_solve(b200_ctx *ctx, const b200_csr *A, const b200_csr *At, void *
 
 int b200_lsmr_solve(b200_ctx *ctx, const b200_csr *A, const b200_csr *At, void *x_dev, const void *b_dev,
                     const b200_lsq_opts *opts, b200_lsq_result *res, double *hist_host, int64_t hist_cap) {
+  B200_TRY(real_only(A, "b200_lsmr_solve"));
+  B200_TRY(real_only(At, "b200_lsmr_solve"));
   B200_TRY(check_ls_args(ctx, A, At, x_dev, b_dev, opts));
   return lsq_dispatch<true>(ctx, CudaOp{A, nullptr}, CudaOp{At, nullptr}, A->dtype, A->m_local, At->m_local,
                             A->m_global, A->n_global, x_dev, b_dev, opts, res, hist_host, hist_cap);
@@ -113,6 +117,8 @@ int b200_lsmr_solve(b200_ctx *ctx, const b200_csr *A, const b200_csr *At, void *
 
 int b200_lsqr_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *At, void *x_dev, const void *b_dev,
                        const b200_lsq_opts *opts, b200_lsq_result *res, double *hist_host, int64_t hist_cap) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_lsqr_solve_op"));
+  B200_TRY(real_only(At ? At->dtype : B200_F64, "b200_lsqr_solve_op"));
   B200_TRY(check_ls_op_args(ctx, A, At, x_dev, b_dev, opts));
   return lsq_dispatch<false>(ctx, CudaOp{nullptr, A}, CudaOp{nullptr, At}, A->dtype, A->m_local, A->n_local,
                              A->m_global, A->n_global, x_dev, b_dev, opts, res, hist_host, hist_cap);
@@ -120,6 +126,8 @@ int b200_lsqr_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *At,
 
 int b200_lsmr_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *At, void *x_dev, const void *b_dev,
                        const b200_lsq_opts *opts, b200_lsq_result *res, double *hist_host, int64_t hist_cap) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_lsmr_solve_op"));
+  B200_TRY(real_only(At ? At->dtype : B200_F64, "b200_lsmr_solve_op"));
   B200_TRY(check_ls_op_args(ctx, A, At, x_dev, b_dev, opts));
   return lsq_dispatch<true>(ctx, CudaOp{nullptr, A}, CudaOp{nullptr, At}, A->dtype, A->m_local, A->n_local,
                             A->m_global, A->n_global, x_dev, b_dev, opts, res, hist_host, hist_cap);

@@ -65,6 +65,7 @@ extern "C" {
 
 int b200_bicgstabl_solve_op(b200_ctx *ctx, const b200_linop *A, void *x_dev, const void *b_dev,
                             const b200_bicgstabl_opts *opts, b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_bicgstabl_solve_op"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts, "NULL argument");
   B200_TRY(check_linop(A, "A"));
   B200_REQUIRE(A->m_global == A->n_global && A->m_local == A->n_local, "bicgstabl! needs a square operator");
@@ -74,6 +75,7 @@ int b200_bicgstabl_solve_op(b200_ctx *ctx, const b200_linop *A, void *x_dev, con
 
 int b200_minres_solve_op(b200_ctx *ctx, const b200_linop *A, void *x_dev, const void *b_dev, const b200_minres_opts *opts,
                          b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_minres_solve_op"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts, "NULL argument");
   B200_TRY(check_linop(A, "A"));
   B200_REQUIRE(A->m_global == A->n_global && A->m_local == A->n_local, "minres! needs a square operator");

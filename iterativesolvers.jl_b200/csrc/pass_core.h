@@ -29,6 +29,8 @@
 #include <stdint.h>
 #include <string.h>
 
+#include "complex.h"
+
 #ifdef __CUDACC__
 #define B200_HD __host__ __device__ __forceinline__
 #define B200_UNROLL _Pragma("unroll")
@@ -44,7 +46,7 @@ constexpr int kPassMaxRed = 16;   // sums per pass (IDR(s) with s <= 16 needs s)
 // machine epsilon of the vector element type (eps(real(T)) of the reference's default tolerances)
 template <typename T>
 B200_HD double eps_of() {
-  return sizeof(T) == 8 ? 2.220446049250313e-16 : 1.1920928955078125e-07;
+  return sizeof(typename real_of<T>::type) == 8 ? 2.220446049250313e-16 : 1.1920928955078125e-07;
 }
 
 // LinearAlgebra.givensAlgorithm(f, g) for real arguments -> (c, s, r) with [c s; -s c][f; g] = [r; 0]

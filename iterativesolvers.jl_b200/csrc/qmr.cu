@@ -39,14 +39,20 @@ int qmr_dispatch(b200_ctx *ctx, const CudaOp &A, const CudaOp &At, int dtype, in
 }  // namespace
 
 namespace b200 {
-// argument check shared by the *_op entry points (linop.cuh)
-int check_linop(const b200_linop *A, const char *what) {
+// argument check of a b200_linop with the complex element types allowed (cg! and gmres! on single-GPU contexts)
+int check_linop_complex(const b200_linop *A, const char *what) {
   B200_REQUIRE(A, "%s is NULL", what);
   B200_REQUIRE(A->apply, "%s: apply callback is NULL", what);
-  B200_REQUIRE(A->dtype == B200_F64 || A->dtype == B200_F32, "%s: bad dtype", what);
+  B200_REQUIRE(A->dtype >= B200_F64 && A->dtype <= B200_CF32, "%s: bad dtype", what);
   B200_REQUIRE(A->m_local >= 0 && A->n_local >= 0 && A->m_global >= A->m_local && A->n_global >= A->n_local,
                "%s: bad dimensions", what);
   return B200_OK;
+}
+// argument check shared by the *_op entry points (linop.cuh): real element types only
+int check_linop(const b200_linop *A, const char *what) {
+  B200_REQUIRE(A, "%s is NULL", what);
+  B200_TRY(real_only(A->dtype, what));
+  return check_linop_complex(A, what);
 }
 }  // namespace b200
 
@@ -54,6 +60,8 @@ extern "C" {
 
 int b200_qmr_solve(b200_ctx *ctx, const b200_csr *A, const b200_csr *At, void *x_dev, const void *b_dev,
                    const b200_qmr_opts *opts, b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
+  B200_TRY(real_only(A, "b200_qmr_solve"));
+  B200_TRY(real_only(At, "b200_qmr_solve"));
   B200_REQUIRE(ctx && A && At && x_dev && b_dev && opts, "NULL argument");
   B200_REQUIRE(A->ctx == ctx && At->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(is_square(A), "qmr! needs a square operator (got %lld x %lld)", (long long)A->m_global,
@@ -67,6 +75,8 @@ int b200_qmr_solve(b200_ctx *ctx, const b200_csr *A, const b200_csr *At, void *x
 
 int b200_qmr_solve_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *At, void *x_dev, const void *b_dev,
                       const b200_qmr_opts *opts, b200_result *res, double *resnorm_host, int64_t resnorm_cap) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_qmr_solve_op"));
+  B200_TRY(real_only(At ? At->dtype : B200_F64, "b200_qmr_solve_op"));
   B200_REQUIRE(ctx && x_dev && b_dev && opts, "NULL argument");
   B200_TRY(check_linop(A, "A"));
   B200_TRY(check_linop(At, "At"));

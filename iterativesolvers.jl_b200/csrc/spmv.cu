@@ -106,6 +106,8 @@ namespace b200 {
 // internal entry used by the solvers (no argument checks)
 int spmv(b200_ctx *ctx, const b200_csr *A, const void *x, void *y) {
   B200_TRY(halo_exchange(ctx, A, x));
+  if (A->dtype == B200_CF64) return launch_spmv<cplx<double>>(ctx, A, x, y);   // complex operators are single-GPU
+  if (A->dtype == B200_CF32) return launch_spmv<cplx<float>>(ctx, A, x, y);
   return A->dtype == B200_F64 ? launch_spmv<double>(ctx, A, x, y) : launch_spmv<float>(ctx, A, x, y);
 }
 // single-GPU only: y = A x unless (*gate & gate_mask) != 0 on the device when the kernel starts (launches that a solver
@@ -126,6 +128,7 @@ int b200_spmv(b200_ctx *ctx, const b200_csr *A, const void *x_dev, void *y_dev) 
 
 int b200_spmm(b200_ctx *ctx, const b200_csr *A, const void *X_dev, int64_t ldx, void *Y_dev, int64_t ldy, int bs) {
   B200_REQUIRE(ctx && A && X_dev && Y_dev && bs >= 1, "bad arguments");
+  B200_TRY(real_only(A, "b200_spmm"));
   B200_REQUIRE(ctx->world == 1, "block SpMM is single-GPU in this version");
   B200_REQUIRE(ldx >= A->n_global && ldy >= A->m_local, "leading dimensions too small: X has size(A,2) rows, Y size(A,1)");
   B200_REQUIRE(X_dev != Y_dev, "mul!(Y, A, X): Y must not alias X");

@@ -24,6 +24,31 @@ __global__ void __launch_bounds__(kRowsThreads) k_spmv_rows(const int *__restric
   epi.template end<kRowsThreads>(red);
 }
 
+// Complex operators (single-GPU, sub-warp form only): x is the whole operand (no halo); VEC = one vector __ldg per
+// gathered element, chosen by the launcher only when x is aligned to 2 sizeof(R), else two scalar loads.
+template <typename R, bool VEC>
+struct XViewC {
+  const cplx<R> *__restrict__ x;
+  __device__ __forceinline__ cplx<R> operator()(int col) const {
+    if constexpr (VEC) {
+      return __ldg(x + col);
+    } else {
+      const R *p = reinterpret_cast<const R *>(x + col);
+      return cplx<R>(__ldg(p), __ldg(p + 1));
+    }
+  }
+};
+
+template <typename R, int LPR, bool VEC, typename Epi>
+__global__ void __launch_bounds__(kRowsThreads) k_spmv_rows_cplx(const int *__restrict__ rowptr, const int *__restrict__ colind,
+                                                                 const cplx<R> *__restrict__ vals, XViewC<R, VEC> xv,
+                                                                 int64_t m, Epi epi) {
+  if (!epi.begin()) return;
+  __shared__ double red[kRowsThreads / 32];
+  spmv_rows<cplx<R>, LPR>(rowptr, colind, vals, xv, m, epi);
+  epi.template end<kRowsThreads>(red);
+}
+
 template <typename T, int LPR, typename Epi>
 __global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
     k_spmv_csr_stream(const int *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
@@ -54,7 +79,23 @@ template <typename T, typename Epi>
 int launch_spmv_fused(b200_ctx *ctx, const b200_csr *A, const void *x, bool peer_halo, const Epi &epi, bool chained) {
   const T *vals = (const T *)A->vals;
   const int64_t m = A->m_local;
-  if (use_band(ctx, A, x)) {
+  if constexpr (is_cplx<T>::value) {
+    // complex operators have neither a band description nor CSR-stream tiles (finish_operator): always the sub-warp form,
+    // whatever "spmv_kernel" asks for.  vals are library-allocated (aligned); x may be a caller's view at any element offset.
+    typedef typename real_of<T>::type R;
+    const bool vec = ((uintptr_t)x % sizeof(T)) == 0;
+    B200_TRY(with_lpr<2>(pick_lpr(A->avg_row_nnz), [&](auto lpr) -> int {
+      constexpr int L = decltype(lpr)::value;
+      const dim3 grid(stream_grid(ctx, m, kRowsThreads / L, 8));
+      if (vec)
+        B200_CUDA(launch_chained(chained, k_spmv_rows_cplx<R, L, true, Epi>, grid, dim3(kRowsThreads), 0, ctx->stream,
+                                 A->rowptr, A->colind, vals, XViewC<R, true>{(const T *)x}, m, epi));
+      else
+        B200_CUDA(launch_chained(chained, k_spmv_rows_cplx<R, L, false, Epi>, grid, dim3(kRowsThreads), 0, ctx->stream,
+                                 A->rowptr, A->colind, vals, XViewC<R, false>{(const T *)x}, m, epi));
+      return B200_OK;
+    }));
+  } else if (use_band(ctx, A, x)) {
     // band descriptions exist on single-GPU contexts only: x is the whole operand, n_global entries (== m for the
     // square operators of the solvers)
     const size_t smem = sizeof(BandSmem<T>);

@@ -86,6 +86,7 @@ extern "C" {
 
 int b200_stationary(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *b_dev, int method, double omega,
                     int64_t maxiter) {
+  B200_TRY(real_only(A, "b200_stationary"));
   B200_REQUIRE(ctx && A && x_dev && b_dev, "NULL argument");
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(ctx->world == 1, "the stationary methods sweep the whole matrix in order: single-GPU contexts only");

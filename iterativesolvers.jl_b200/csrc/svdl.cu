@@ -63,6 +63,8 @@ extern "C" {
 int b200_svdl(b200_ctx *ctx, const b200_csr *A, const b200_csr *At, const void *v0_dev, const b200_svdl_opts *opts,
               b200_svdl_result *res, double *sigma_host, void *U_dev, int64_t ldu, void *V_dev, int64_t ldv,
               double *hist_ritz, double *hist_resnorm, int32_t *hist_conv, double *hist_betas, double *B_host) {
+  B200_TRY(real_only(A, "b200_svdl"));
+  B200_TRY(real_only(At, "b200_svdl"));
   B200_REQUIRE(ctx && A && At && v0_dev && opts && sigma_host, "NULL argument");
   B200_REQUIRE(A->ctx == ctx && At->ctx == ctx && At->dtype == A->dtype, "operators must share context and element type");
   if (ctx->world == 1) {
@@ -80,6 +82,8 @@ int b200_svdl_op(b200_ctx *ctx, const b200_linop *A, const b200_linop *At, const
                  const b200_svdl_opts *opts, b200_svdl_result *res, double *sigma_host, void *U_dev, int64_t ldu,
                  void *V_dev, int64_t ldv, double *hist_ritz, double *hist_resnorm, int32_t *hist_conv,
                  double *hist_betas, double *B_host) {
+  B200_TRY(real_only(A ? A->dtype : B200_F64, "b200_svdl_op"));
+  B200_TRY(real_only(At ? At->dtype : B200_F64, "b200_svdl_op"));
   B200_REQUIRE(ctx && v0_dev && opts && sigma_host, "NULL argument");
   B200_TRY(check_linop(A, "A"));
   B200_TRY(check_linop(At, "At"));

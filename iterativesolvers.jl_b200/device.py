@@ -8,14 +8,22 @@ import numpy as np
 from . import _lib
 from ._lib import check, lib
 
-_DT = {np.dtype(np.float64): _lib.F64, np.dtype(np.float32): _lib.F32}
+_DT = {np.dtype(np.float64): _lib.F64, np.dtype(np.float32): _lib.F32,
+       np.dtype(np.complex128): _lib.CF64, np.dtype(np.complex64): _lib.CF32}
+_DT_OF_CODE = {code: dt for dt, code in _DT.items()}
 
 
 def dtype_code(dt) -> int:
     dt = np.dtype(dt)
     if dt not in _DT:
-        raise TypeError(f"unsupported element type {dt}: the device path handles Float64 and Float32")
+        raise TypeError(f"unsupported element type {dt}: the device path handles Float64, Float32, ComplexF64 and "
+                        "ComplexF32")
     return _DT[dt]
+
+
+def dtype_of_code(code: int) -> np.dtype:
+    """the numpy dtype of a B200_* element type code"""
+    return _DT_OF_CODE[int(code)]
 
 
 class Context:

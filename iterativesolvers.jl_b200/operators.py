@@ -8,7 +8,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import check, lib
-from .device import Context, DeviceArray, as_device_ptr, default_context, dtype_code
+from .device import Context, DeviceArray, as_device_ptr, default_context, dtype_code, dtype_of_code
 
 
 def _vp(a: np.ndarray):
@@ -132,7 +132,7 @@ class B200CSR:
         rb, nh = C.c_int64(), C.c_int64()
         check(lib().b200_csr_info(handle, C.byref(m), C.byref(n), C.byref(nnz), C.byref(dt), C.byref(rb), C.byref(nh)))
         self.m_local, self.n_global, self.nnz, self.row_begin, self.n_halo = m.value, n.value, nnz.value, rb.value, nh.value
-        self.dtype = np.dtype(np.float64 if dt.value == _lib.F64 else np.float32)
+        self.dtype = dtype_of_code(dt.value)
         self.code = dt.value
         # size(A, 1): row-partitioned (multi-GPU) operators are square; single-GPU ones may be rectangular (lsqr!/lsmr!)
         self.m_global = self.m_local if ctx.world == 1 else self.n_global

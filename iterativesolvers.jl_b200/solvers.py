@@ -17,7 +17,7 @@ import numpy as np
 
 from . import _lib
 from ._lib import B200Error, check, lib
-from .device import DeviceArray, as_device_ptr, is_device
+from .device import DeviceArray, as_device_ptr, dtype_code, is_device
 from .history import ConvergenceHistory
 from .operators import B200CSR, B200LinearOperator, FunctionPrec, Identity, precond_to_c
 
@@ -985,7 +985,7 @@ class LobpcgConstraint:
             Yd = Y if is_device(Y) else DeviceArray.from_numpy(ctx, np.asfortranarray(Y, dtype=self.dtype))
             if Yd.shape[0] != self.n:
                 raise ValueError("the constraint must have as many rows as the operator")
-        code = _lib.F64 if self.dtype == np.float64 else _lib.F32
+        code = dtype_code(self.dtype)
         if B is not None:                                      # Constraint(Y, B, X) with BY = B*Y  src/lobpcg.jl:161-186
             bs, bop = _linop_struct(B)
             self._keep, self._bop = (bs, B), bop               # append applies B again (update!, :188-206)
