@@ -20,6 +20,9 @@
               gmres!(30, CGS) on the shifted Helmholtz operator -Laplace - k^2 I + i sigma I, and cg! on the Hermitian
               positive-definite L + I + i S (S the antisymmetric central difference in x, coefficient 1/4); fixed
               iteration counts; one JSON line each with it/s, the complex SpMV's ms per launch and its GB/s
+    large     (command line only) an operator above 2^31 nonzeros: laplace_matrix(Float64, 680, 3) built on the device
+              (2 198 249 600 nonzeros, 8-byte row offsets): cg! it/s and mul!'s ms per launch and GB/s.  Prints a
+              "skipped" record instead when the GPU has too little free memory (about 47 GiB are needed)
 
 Each line is a JSON object with iterations/s, per-kernel-class CUDA-event times recorded inside the run
 (b200_ctx_profile_*), the algorithmic bytes (SURVEY.md section 8d) and the achieved fraction of the measured
@@ -480,10 +483,61 @@ def run_complex(grid=256, iters=None, reps=2, ctx=None):
     return out
 
 
+def run_large(grid=680, iters=None, reps=2, ctx=None):
+    """the `large` workload: cg! and mul! on laplace_matrix(Float64, grid, 3) with 8-byte row offsets"""
+    import torch
+    import iterativesolvers_jl_b200 as isb
+    n = grid ** 3
+    nnz = n + 6 * (grid - 1) * grid * grid
+    V = 8
+    free, _ = torch.cuda.mem_get_info(0)
+    need = nnz * (V + 4) + (n + 1) * 8 + 6 * n * V          # operator + cg!'s x, b, r, u, c and mul!'s y
+    gpu = gpu_name_power(0)
+    if need > 0.95 * free:
+        return {"config": "large", "grid": grid, "skipped": f"needs {need / 2**30:.1f} GiB of free device memory, "
+                f"{free / 2**30:.1f} GiB are free", **gpu}
+    ctx = ctx or isb.default_context()
+    L = isb.lib()
+    A = isb.B200CSR.laplacian(grid, 3, np.float64, ctx=ctx)
+    kind, sbytes = C.c_int(), C.c_int64()
+    L.b200_csr_stream_kind(A._h, C.byref(kind), C.byref(sbytes))
+    csr_b = nnz * (V + 4) + (n + 1) * 8 + 2 * n * V           # algorithmic bytes of one SpMV (SURVEY 8d, 8-byte offsets)
+    read_b = nnz * V + sbytes.value + 2 * n * V               # what the chosen form reads: vals, its structure, x, y
+    rng = np.random.default_rng(1234321)
+    b = rng.standard_normal(n)
+    b /= np.linalg.norm(b)
+    bd = isb.DeviceArray.from_numpy(ctx, b)
+    del b
+    xd = isb.DeviceArray.zeros(ctx, n, np.float64)
+    yd = isb.DeviceArray.zeros(ctx, n, np.float64)
+    it = iters or 200
+    for rep in range(reps + 1):
+        L.b200_fill(ctx._h, n, 0.0, xd._p, isb._lib.F64)
+        ctx.sync()
+        t0 = time.perf_counter()
+        x, h = isb.cg_(xd, A, bd, maxiter=it, initially_zero=True, log=True, reltol=0.0)
+        ctx.sync()
+        dt = time.perf_counter() - t0
+    K = 50
+    A.mul_(yd, bd)
+    ctx.timer_start()
+    for _ in range(K):
+        A.mul_(yd, bd)
+    spmv_ms = ctx.timer_stop() / K
+    rec = {"config": "large", "solver": "cg! and mul!, laplace_matrix(Float64, 680, 3), 8-byte row offsets", "grid": grid,
+           "n": n, "nnz": A.nnz, "index_bytes": A.index_bytes, "stream_kind": kind.value, **gpu,
+           "iters": h.niters, "seconds": dt, "iters_per_s": h.niters / dt,
+           "resnorm_first_last": [float(h["resnorm"][0]), float(h["resnorm"][-1])],
+           "spmv_ms_per_launch": spmv_ms, "spmv_bytes_algorithmic": csr_b, "spmv_bytes_read": read_b,
+           "spmv_gbs_algorithmic": csr_b / (spmv_ms * 1e-3) / 1e9, "spmv_gbs_read": read_b / (spmv_ms * 1e-3) / 1e9}
+    A.close()
+    return rec
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", choices=["gmres", "lobpcg", "minres", "bicgstabl", "cg256", "widen", "general", "scattered", "cg2d",
-                                      "complex"])
+                                      "complex", "large"])
     ap.add_argument("--grid", type=int, default=256)
     ap.add_argument("--iters", type=int, default=None)
     ap.add_argument("--orth", default="cgs")
@@ -493,6 +547,9 @@ def main():
     args = ap.parse_args()
     import torch
     torch.cuda.set_device(0)
+    if args.which == "large":
+        print(json.dumps(run_large(680 if args.grid == 256 else args.grid, args.iters, args.reps)))
+        return
     if args.which == "complex":
         for rec in run_complex(args.grid, args.iters, args.reps):
             print(json.dumps(rec))

@@ -133,7 +133,13 @@ B200_API int b200_ctx_profile_read(b200_ctx *ctx, int slot, double *total_ms, in
  *           next kernel's blocks are resident when the previous one ends; 0 (default) = plain stream order
  *   "cg_persistent": 1 (default) = cg! on single-GPU operators of at most 2^18 rows runs its whole loop in ONE persistent
  *           cooperative kernel (grid-wide barriers between the phases of an iteration instead of three launches; same
- *           recurrence, same operation order); 0 = the streaming three-kernel iteration at every size
+ *           recurrence, same operation order); 0 = the streaming three-kernel iteration at every size.  Operators with
+ *           8-byte row offsets (see "rowptr64") always take the streaming iteration: the persistent kernel reads 4-byte ones
+ *   "rowptr64": width of the row offsets of the single-GPU operators built on this context afterwards (b200_csr_from_csc,
+ *           _from_csr_slab, _laplacian, _transpose keeps its argument's width): 0 (default) = 8 bytes when nnz >= 2^31 - 1,
+ *           else 4 bytes; 1 = always 8 bytes (same results bit for bit; lets small operators exercise the 8-byte
+ *           kernels).  Column indices stay int32 (n < 2^31), and multi-GPU slabs always have 4-byte offsets.  See
+ *           b200_csr_index_bytes and b200_csr_download64; b200_stationary refuses 8-byte operators
  *   "fold_push": 1 (default) = multi-GPU peer-memory cg! with Identity: the kernel that updates r stores r's boundary rows
  *           into the neighbours' halo segments itself and its finishing block raises the halo flags (one launch less
  *           per iteration; needs one contiguous row range per neighbour); 0 = separate push kernel
@@ -189,12 +195,18 @@ B200_API int b200_csr_transpose(b200_ctx *ctx, const b200_csr *A, b200_csr **out
  * kind 3 = band stream (a single-GPU operator whose 512-row tiles each have at most 8 distinct diagonal offsets
  * col - row and whose rows have strictly ascending columns: per tile its offsets, per row one mask byte),
  * 2 = CSR stream, 1 = sub-warp-per-row kernel (always for complex operators).  structure_bytes = bytes of structure (everything but vals and the
- * vectors) that form reads per SpMV: 576 per 512-row tile for the band stream, 4*nnz + 4*(rows+1) for CSR. */
+ * vectors) that form reads per SpMV: 576 per 512-row tile for the band stream, 4*nnz + b*(rows+1) for CSR, b = 4 or 8
+ * the width of the row offsets (b200_csr_index_bytes). */
 B200_API int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes);
 /* diag(A) of the local rows into a device vector (JacobiPrec(diag(A)), reference test/cg.jl:57) */
 B200_API int b200_csr_diag(b200_ctx *ctx, const b200_csr *A, void *diag_dev);
-/* device CSR arrays back to the host (tests) */
+/* device CSR arrays back to the host (tests).  B200_ERR_UNSUPPORTED for an operator with 8-byte row offsets: use
+ * b200_csr_download64, which takes either width. */
 B200_API int b200_csr_download(b200_ctx *ctx, const b200_csr *A, int32_t *rowptr, int32_t *colind, void *vals);
+B200_API int b200_csr_download64(b200_ctx *ctx, const b200_csr *A, int64_t *rowptr, int32_t *colind, void *vals);
+/* width of the operator's row offsets in bytes: 4, or 8 (single-GPU operators with nnz >= 2^31 - 1, or built with the
+ * context option "rowptr64" = 1) */
+B200_API int b200_csr_index_bytes(const b200_csr *A, int *bytes);
 
 /* Host-side halo plan for row-partitioned operators (multi-GPU).  Pure host code: usable (and
  * tested) without a GPU.  row_offsets has world+1 entries (rank r owns [row_offsets[r], row_offsets[r+1])). */

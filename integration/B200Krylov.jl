@@ -126,6 +126,19 @@ function Base.adjoint(A::B200CSR{T}) where {T}
 end
 mul!(y::B200Vector{T}, A::B200CSR{T}, x::B200Vector{T}) where {T} =
     (check(ccall((:b200_spmv, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}), A.ctx.h, A.h, x.p, y.p)); y)
+# the device operator back as a SparseMatrixCSC{T,Int64}: its CSR is the CSC of transpose(A) (no conjugation).  Row
+# offsets come through b200_csr_download64, which serves 4-byte and 8-byte operators alike.
+function SparseArrays.SparseMatrixCSC(A::B200CSR{T}) where {T}
+    nnz = Ref{Int64}(0)
+    check(ccall((:b200_csr_info, LIB), Cint, (Ptr{Cvoid}, Ptr{Int64}, Ptr{Int64}, Ref{Int64}, Ptr{Cint}, Ptr{Int64}, Ptr{Int64}),
+                A.h, C_NULL, C_NULL, nnz, C_NULL, C_NULL, C_NULL))
+    rowptr = Vector{Int64}(undef, A.n + 1)
+    colind = Vector{Int32}(undef, nnz[])
+    vals = Vector{T}(undef, nnz[])
+    check(ccall((:b200_csr_download64, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Int64}, Ptr{Int32}, Ptr{T}),
+                A.ctx.h, A.h, rowptr, colind, vals))
+    transpose(SparseMatrixCSC(A.ncols, A.n, rowptr .+ 1, Int64.(colind) .+ 1, vals)) |> SparseMatrixCSC
+end
 
 # the diagonal preconditioner of test/cg.jl:14-18
 struct JacobiPrec{T}

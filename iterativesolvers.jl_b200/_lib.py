@@ -152,6 +152,8 @@ SIGNATURES = {
     "b200_csr_stream_kind": (_INT, [_P, C.POINTER(_INT), C.POINTER(_I64)]),
     "b200_csr_diag": (_INT, [_P, _P, _P]),
     "b200_csr_download": (_INT, [_P, _P, _P, _P, _P]),
+    "b200_csr_download64": (_INT, [_P, _P, _P, _P, _P]),
+    "b200_csr_index_bytes": (_INT, [_P, C.POINTER(_INT)]),
     "b200_halo_plan_create": (_INT, [_INT, _INT, C.POINTER(_I64), C.POINTER(_P)]),
     "b200_halo_plan_scan": (_INT, [_P, _I64, _P, _P, _INT, _INT]),
     "b200_halo_plan_scan_laplacian": (_INT, [_P, _I64, _INT]),

@@ -647,7 +647,8 @@ int cg_setup(CgEngine<T> &e, b200_ctx *ctx, const b200_csr *A, T *x, const T *b,
   e.fold_halo = e.mode == COMM_PEER && !e.jac && A->halo && A->halo_peer && A->n_halo > 0;
   if (e.fold_halo) B200_CUDA(cudaMemsetAsync(A->halo, 0, sizeof(T) * (size_t)A->n_halo, st));   // u_0 = 0
   e.persistent = false;
-  if (ctx->world == 1 && ctx->opt_cg_persistent != 0 && n > 0 && n <= kPersistMaxRows) {
+  // k_cg_persistent reads 4-byte row offsets only: an operator with 8-byte offsets takes the streaming iteration
+  if (ctx->world == 1 && ctx->opt_cg_persistent != 0 && n > 0 && n <= kPersistMaxRows && A->rowptr) {
     int per_sm = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cg_persistent_kernel<T>(e.lpr), kThreads, 0) == cudaSuccess &&
         per_sm >= 1) {

@@ -103,6 +103,7 @@ struct b200_ctx {
                                  // wgmma (lobpcg_gram_wgmma.cuh), 2 = legacy mma.sync Gram, 0 = SIMT kernels
   int opt_orth_fused = 1;        // b200_ctx_set_option("orth_fused"): 1 = one cooperative launch per CGS/DGKS orthogonalisation and a
                                  // device-resident GMRES cycle (single GPU); 0 = the three-kernel path with host-side recurrences
+  int opt_rowptr64 = 0;          // b200_ctx_set_option("rowptr64"): 0 = 8-byte row offsets when nnz >= INT32_MAX, 1 = always (single GPU)
   int opt_cg_persistent = 1;     // b200_ctx_set_option("cg_persistent"): operators of <= 2^18 rows run the whole cg! loop in one cooperative kernel
   int opt_fold_push = 1;         // b200_ctx_set_option("fold_push"): peer path, cg! with Identity: K3 stores r's boundary rows to the neighbours itself
   int opt_pdl = 0;               // b200_ctx_set_option("pdl"): chain the kernels of a CG iteration with programmatic dependent launch

@@ -1,5 +1,8 @@
-// csr.cu -- building the device operator: SparseMatrixCSC -> CSR int32 (device transpose),
-// CSR row slabs, the on-device laplace_matrix generator, halo plans and the halo exchange.
+// csr.cu -- building the device operator: SparseMatrixCSC -> CSR (device transpose), CSR row slabs, the on-device
+// laplace_matrix generator, halo plans and the halo exchange.
+//
+// Row offsets are int32, or int64 for single-GPU operators of INT32_MAX or more nonzeros (csr.cuh).  Every kernel that
+// reads or writes them has an overload per width around one shared body (spmv_launch.cuh says why overloads).
 #include <algorithm>
 #include <cub/cub.cuh>
 
@@ -149,23 +152,37 @@ int b200_halo_plan_destroy(b200_halo_plan *p) {
 // ------------------------------------------------------------------------------------------
 namespace {
 
-template <typename I>
-__global__ void k_count_rows(const I *__restrict__ rowval, int64_t nnz, int base, int64_t m, int *__restrict__ cnt,
-                             int *__restrict__ err) {
+__device__ __forceinline__ void count_one(int *c) { atomicAdd(c, 1); }
+__device__ __forceinline__ void count_one(int64_t *c) { atomicAdd((unsigned long long *)c, 1ull); }
+
+template <typename I, typename P>
+__device__ __forceinline__ void count_rows(const I *__restrict__ rowval, int64_t nnz, int base, int64_t m,
+                                           P *__restrict__ cnt, int *__restrict__ err) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < nnz; k += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = (int64_t)rowval[k] - base;
     if (r < 0 || r >= m) {
       *err = 1;
       continue;
     }
-    atomicAdd(&cnt[r], 1);
+    count_one(&cnt[r]);
   }
+}
+template <typename I>
+__global__ void k_count_rows(const I *__restrict__ rowval, int64_t nnz, int base, int64_t m, int *__restrict__ cnt,
+                             int *__restrict__ err) {
+  count_rows(rowval, nnz, base, m, cnt, err);
+}
+template <typename I>
+__global__ void k_count_rows(const I *__restrict__ rowval, int64_t nnz, int base, int64_t m, int64_t *__restrict__ cnt,
+                             int *__restrict__ err) {
+  count_rows(rowval, nnz, base, m, cnt, err);
 }
 
 // expand colptr into a per-nonzero column id and the row key used by the stable sort
-template <typename I>
-__global__ void k_expand_cols(const I *__restrict__ colptr, int64_t n, int base, const I *__restrict__ rowval,
-                              unsigned int *__restrict__ key_row, int *__restrict__ col_of) {
+template <typename IC, typename IR>
+__device__ __forceinline__ void expand_cols(const IC *__restrict__ colptr, int64_t n, int base,
+                                            const IR *__restrict__ rowval, unsigned int *__restrict__ key_row,
+                                            int *__restrict__ col_of) {
   // one warp per column (columns are short); lanes stride the column's entries
   const int64_t warp = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -178,21 +195,55 @@ __global__ void k_expand_cols(const I *__restrict__ colptr, int64_t n, int base,
     }
   }
 }
+template <typename I>
+__global__ void k_expand_cols(const I *__restrict__ colptr, int64_t n, int base, const I *__restrict__ rowval,
+                              unsigned int *__restrict__ key_row, int *__restrict__ col_of) {
+  expand_cols(colptr, n, base, rowval, key_row, col_of);
+}
+// the CSC of the adjoint of an operator with 8-byte row offsets: int64 colptr, int32 rowval
+__global__ void k_expand_cols(const int64_t *__restrict__ colptr, int64_t n, int base, const int *__restrict__ rowval,
+                              unsigned int *__restrict__ key_row, int *__restrict__ col_of) {
+  expand_cols(colptr, n, base, rowval, key_row, col_of);
+}
 
-template <typename T, typename TI>
-__global__ void k_gather_vals(const int *__restrict__ perm, const TI *__restrict__ nz_in, int64_t nnz,
-                              T *__restrict__ vals) {
+// perm: int, or int64_t when the operator has 8-byte row offsets (positions up to nnz)
+template <typename T, typename TI, typename P>
+__device__ __forceinline__ void gather_vals(const P *__restrict__ perm, const TI *__restrict__ nz_in, int64_t nnz,
+                                            T *__restrict__ vals) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < nnz; k += (int64_t)gridDim.x * blockDim.x)
     vals[k] = (T)nz_in[perm[k]];
 }
-__global__ void k_gather_int(const int *__restrict__ perm, const int *__restrict__ in, int64_t nnz,
-                             int *__restrict__ out) {
+template <typename T, typename TI>
+__global__ void k_gather_vals(const int *__restrict__ perm, const TI *__restrict__ nz_in, int64_t nnz,
+                              T *__restrict__ vals) {
+  gather_vals(perm, nz_in, nnz, vals);
+}
+template <typename T, typename TI>
+__global__ void k_gather_vals(const int64_t *__restrict__ perm, const TI *__restrict__ nz_in, int64_t nnz,
+                              T *__restrict__ vals) {
+  gather_vals(perm, nz_in, nnz, vals);
+}
+template <typename P>
+__device__ __forceinline__ void gather_int(const P *__restrict__ perm, const int *__restrict__ in, int64_t nnz,
+                                           int *__restrict__ out) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < nnz; k += (int64_t)gridDim.x * blockDim.x)
     out[k] = in[perm[k]];
+}
+__global__ void k_gather_int(const int *__restrict__ perm, const int *__restrict__ in, int64_t nnz,
+                             int *__restrict__ out) {
+  gather_int(perm, in, nnz, out);
+}
+__global__ void k_gather_int(const int64_t *__restrict__ perm, const int *__restrict__ in, int64_t nnz,
+                             int *__restrict__ out) {
+  gather_int(perm, in, nnz, out);
 }
 __global__ void k_iota(int *p, int64_t n) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x)
     p[k] = (int)k;
+}
+__global__ void k_iota(int64_t *p, int64_t n) {
+  for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x)
+    p[k] = k;
 }
 
 // CSR slab: global column -> local extended index (binary search of the sorted halo list)
@@ -220,11 +271,19 @@ __global__ void k_remap_cols(const I *__restrict__ col_in, int64_t nnz, int base
   }
 }
 
-template <typename I>
-__global__ void k_rowptr_convert(const I *__restrict__ in, int64_t m, int *__restrict__ out) {
+template <typename I, typename P>
+__device__ __forceinline__ void rowptr_convert(const I *__restrict__ in, int64_t m, P *__restrict__ out) {
   const I first = in[0];
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k <= m; k += (int64_t)gridDim.x * blockDim.x)
-    out[k] = (int)(in[k] - first);
+    out[k] = (P)(in[k] - first);
+}
+template <typename I>
+__global__ void k_rowptr_convert(const I *__restrict__ in, int64_t m, int *__restrict__ out) {
+  rowptr_convert(in, m, out);
+}
+template <typename I>
+__global__ void k_rowptr_convert(const I *__restrict__ in, int64_t m, int64_t *__restrict__ out) {
+  rowptr_convert(in, m, out);
 }
 
 template <typename T, typename TI>
@@ -239,7 +298,8 @@ struct LapGeom {
   int dims;
   int64_t stride[6];
 };
-__global__ void k_lap_count(LapGeom g, int64_t row_begin, int64_t m, int *__restrict__ cnt) {
+template <typename P>
+__device__ __forceinline__ void lap_count(LapGeom g, int64_t row_begin, int64_t m, P *__restrict__ cnt) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
     int64_t q = row_begin + i, rem = q;
     int c = 1;
@@ -251,10 +311,16 @@ __global__ void k_lap_count(LapGeom g, int64_t row_begin, int64_t m, int *__rest
     cnt[i] = c;
   }
 }
-template <typename T>
-__global__ void k_lap_fill(LapGeom g, int64_t row_begin, int64_t m, const int *__restrict__ rowptr,
-                           const int64_t *__restrict__ halo_sorted, int64_t n_halo, int *__restrict__ colind,
-                           T *__restrict__ vals) {
+__global__ void k_lap_count(LapGeom g, int64_t row_begin, int64_t m, int *__restrict__ cnt) {
+  lap_count(g, row_begin, m, cnt);
+}
+__global__ void k_lap_count(LapGeom g, int64_t row_begin, int64_t m, int64_t *__restrict__ cnt) {
+  lap_count(g, row_begin, m, cnt);
+}
+template <typename T, typename I>
+__device__ __forceinline__ void lap_fill(LapGeom g, int64_t row_begin, int64_t m, const I *__restrict__ rowptr,
+                                         const int64_t *__restrict__ halo_sorted, int64_t n_halo,
+                                         int *__restrict__ colind, T *__restrict__ vals) {
   const int64_t lo = row_begin, hi = row_begin + m;
   auto local = [&](int64_t c) -> int {
     if (c >= lo && c < hi) return (int)(c - lo);
@@ -272,7 +338,7 @@ __global__ void k_lap_fill(LapGeom g, int64_t row_begin, int64_t m, const int *_
       coord[d] = rem % g.N;
       rem /= g.N;
     }
-    int k = rowptr[i];
+    I k = rowptr[i];
     for (int d = g.dims - 1; d >= 0; --d)
       if (coord[d] > 0) {
         colind[k] = local(q - g.stride[d]);
@@ -290,36 +356,75 @@ __global__ void k_lap_fill(LapGeom g, int64_t row_begin, int64_t m, const int *_
       }
   }
 }
-
 template <typename T>
-__global__ void k_diag(const int *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
-                       int64_t m, T *__restrict__ diag) {
+__global__ void k_lap_fill(LapGeom g, int64_t row_begin, int64_t m, const int *__restrict__ rowptr,
+                           const int64_t *__restrict__ halo_sorted, int64_t n_halo, int *__restrict__ colind,
+                           T *__restrict__ vals) {
+  lap_fill(g, row_begin, m, rowptr, halo_sorted, n_halo, colind, vals);
+}
+template <typename T>
+__global__ void k_lap_fill(LapGeom g, int64_t row_begin, int64_t m, const int64_t *__restrict__ rowptr,
+                           const int64_t *__restrict__ halo_sorted, int64_t n_halo, int *__restrict__ colind,
+                           T *__restrict__ vals) {
+  lap_fill(g, row_begin, m, rowptr, halo_sorted, n_halo, colind, vals);
+}
+
+template <typename T, typename I>
+__device__ __forceinline__ void diag_rows(const I *__restrict__ rowptr, const int *__restrict__ colind,
+                                          const T *__restrict__ vals, int64_t m, T *__restrict__ diag) {
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
     T d = (T)0;
-    for (int k = rowptr[i]; k < rowptr[i + 1]; ++k)
+    for (I k = rowptr[i]; k < rowptr[i + 1]; ++k)
       if (colind[k] == (int)i) d += vals[k];
     diag[i] = d;
   }
 }
+template <typename T>
+__global__ void k_diag(const int *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
+                       int64_t m, T *__restrict__ diag) {
+  diag_rows(rowptr, colind, vals, m, diag);
+}
+template <typename T>
+__global__ void k_diag(const int64_t *__restrict__ rowptr, const int *__restrict__ colind, const T *__restrict__ vals,
+                       int64_t m, T *__restrict__ diag) {
+  diag_rows(rowptr, colind, vals, m, diag);
+}
 
-__global__ void k_row_stats(const int *__restrict__ rowptr, int64_t m, int *__restrict__ max_len) {
+// row lengths are < 2^31 (columns are int32) at either offset width
+template <typename I>
+__device__ __forceinline__ void row_stats(const I *__restrict__ rowptr, int64_t m, int *__restrict__ max_len) {
   int local = 0;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x)
-    local = max(local, rowptr[i + 1] - rowptr[i]);
+    local = max(local, (int)(rowptr[i + 1] - rowptr[i]));
   for (int o = 16; o > 0; o >>= 1) local = max(local, __shfl_xor_sync(0xffffffffu, local, o));
   if ((threadIdx.x & 31) == 0) atomicMax(max_len, local);
 }
+__global__ void k_row_stats(const int *__restrict__ rowptr, int64_t m, int *__restrict__ max_len) {
+  row_stats(rowptr, m, max_len);
+}
+__global__ void k_row_stats(const int64_t *__restrict__ rowptr, int64_t m, int *__restrict__ max_len) {
+  row_stats(rowptr, m, max_len);
+}
 
-// max over uniform tiles of R rows of the tile's nonzero count
-__global__ void k_tile_max(const int *__restrict__ rowptr, int64_t m, int R, int *__restrict__ out) {
+// max over uniform tiles of R rows of the tile's nonzero count, clamped to INT_MAX (only counts <= 4096 matter)
+template <typename I>
+__device__ __forceinline__ void tile_max(const I *__restrict__ rowptr, int64_t m, int R, int *__restrict__ out) {
   const int64_t ntiles = (m + R - 1) / R;
   int local = 0;
   for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < ntiles; t += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r0 = t * R, r1 = (r0 + R < m) ? r0 + R : m;
-    local = max(local, rowptr[r1] - rowptr[r0]);
+    const I c = rowptr[r1] - rowptr[r0];
+    if constexpr (sizeof(I) == 8) local = max(local, (int)(c < INT_MAX ? c : INT_MAX));
+    else local = max(local, c);
   }
   for (int o = 16; o > 0; o >>= 1) local = max(local, __shfl_xor_sync(0xffffffffu, local, o));
   if ((threadIdx.x & 31) == 0) atomicMax(out, local);
+}
+__global__ void k_tile_max(const int *__restrict__ rowptr, int64_t m, int R, int *__restrict__ out) {
+  tile_max(rowptr, m, R, out);
+}
+__global__ void k_tile_max(const int64_t *__restrict__ rowptr, int64_t m, int R, int *__restrict__ out) {
+  tile_max(rowptr, m, R, out);
 }
 
 // Band description (csr.cuh, spmv_stream.cuh): one block per tile of R = kBandTileRows rows, two rows per thread (r0+lt,
@@ -327,9 +432,9 @@ __global__ void k_tile_max(const int *__restrict__ rowptr, int64_t m, int R, int
 // one" (a block minimum); each round also sets that offset's bit in the masks of the rows that have it.  A ninth offset,
 // a row of more than 8 nonzeros or a row whose columns do not strictly ascend sets *bad: the operator keeps the CSR stream.
 constexpr int kBandBuildThreads = kBandTileRows / 2;
-__global__ void __launch_bounds__(kBandBuildThreads)
-    k_band_build(const int *__restrict__ rowptr, const int *__restrict__ colind, int64_t m,
-                 b200_band_tile *__restrict__ hdr, uint8_t *__restrict__ mask, int *bad) {
+template <typename I>
+__device__ __forceinline__ void band_build(const I *__restrict__ rowptr, const int *__restrict__ colind, int64_t m,
+                                           b200_band_tile *__restrict__ hdr, uint8_t *__restrict__ mask, int *bad) {
   constexpr int R = kBandTileRows, H = kBandBuildThreads;
   static_assert(2 * H == R, "two rows per thread");
   __shared__ int red[2][H / 32];
@@ -342,7 +447,7 @@ __global__ void __launch_bounds__(kBandBuildThreads)
 #pragma unroll
     for (int q = 0; q < 2; ++q) {
       const int64_t r = r0 + lt + q * H;
-      int b = 0, e = 0;
+      I b = 0, e = 0;
       if (r < m) {
         b = rowptr[r];
         e = rowptr[r + 1];
@@ -396,12 +501,24 @@ __global__ void __launch_bounds__(kBandBuildThreads)
     for (int q = 0; q < 2; ++q) mask[r0 + lt + q * H] = (uint8_t)mk[q];   // 0 for the rows past m of the last tile
     if (lt < 8 && lt >= nb) hdr[t].off[lt] = 0;
     if (lt == 0) {
+      const I k0 = rowptr[r0];
       hdr[t].nb = nb;
-      hdr[t].k0 = rowptr[r0];
-      hdr[t].k1 = rowptr[r0 + R < m ? r0 + R : m];
+      hdr[t].k0 = (int)k0;
+      hdr[t].k1 = (int)rowptr[r0 + R < m ? r0 + R : m];
       for (int p = 0; p < 5; ++p) hdr[t].pad[p] = 0;
+      if constexpr (sizeof(I) == 8) hdr[t].pad[0] = (int)(k0 >> 32);   // the header layout (csr.cuh)
     }
   }
+}
+__global__ void __launch_bounds__(kBandBuildThreads)
+    k_band_build(const int *__restrict__ rowptr, const int *__restrict__ colind, int64_t m,
+                 b200_band_tile *__restrict__ hdr, uint8_t *__restrict__ mask, int *bad) {
+  band_build(rowptr, colind, m, hdr, mask, bad);
+}
+__global__ void __launch_bounds__(kBandBuildThreads)
+    k_band_build(const int64_t *__restrict__ rowptr, const int *__restrict__ colind, int64_t m,
+                 b200_band_tile *__restrict__ hdr, uint8_t *__restrict__ mask, int *bad) {
+  band_build(rowptr, colind, m, hdr, mask, bad);
 }
 
 template <typename T>
@@ -422,7 +539,10 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
   int *d_max = (int *)ctx->d_scalars;  // reuse scratch (int view)
   B200_CUDA(cudaMemsetAsync(d_max, 0, sizeof(int), ctx->stream));
   if (A->m_local > 0) {
-    k_row_stats<<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->m_local, d_max);
+    with_rowptr(A, [&](auto rp) {
+      k_row_stats<<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(rp, A->m_local, d_max);
+      return 0;
+    });
     B200_LAUNCH_CHECK(ctx);
   }
   B200_CUDA(cudaMemcpyAsync(ctx->h_flags, d_max, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
@@ -435,7 +555,10 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
   if (A->m_local > 0 && !is_complex_dtype(A->dtype)) {
     for (int l = 0; l < 6; ++l) {
       B200_CUDA(cudaMemsetAsync(d_max + 1 + l, 0, sizeof(int), ctx->stream));
-      k_tile_max<<<grid_for(ctx, (A->m_local + 15) / 16), 256, 0, ctx->stream>>>(A->rowptr, A->m_local, 512 >> l, d_max + 1 + l);
+      with_rowptr(A, [&](auto rp) {
+        k_tile_max<<<grid_for(ctx, (A->m_local + 15) / 16), 256, 0, ctx->stream>>>(rp, A->m_local, 512 >> l, d_max + 1 + l);
+        return 0;
+      });
       B200_LAUNCH_CHECK(ctx);
     }
     B200_CUDA(cudaMemcpyAsync(ctx->h_flags, d_max + 1, sizeof(int) * 6, cudaMemcpyDeviceToHost, ctx->stream));
@@ -455,8 +578,11 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
     B200_CUDA(cudaMalloc(&A->band_mask, (size_t)kBandTileRows * ntiles));
     int *d_bad = d_max + 7;
     B200_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), ctx->stream));
-    k_band_build<<<grid_for(ctx, ntiles, 1), kBandBuildThreads, 0, ctx->stream>>>(A->rowptr, A->colind, A->m_local,
-                                                                                   A->band_hdr, A->band_mask, d_bad);
+    with_rowptr(A, [&](auto rp) {
+      k_band_build<<<grid_for(ctx, ntiles, 1), kBandBuildThreads, 0, ctx->stream>>>(rp, A->colind, A->m_local,
+                                                                                     A->band_hdr, A->band_mask, d_bad);
+      return 0;
+    });
     B200_LAUNCH_CHECK(ctx);
     B200_CUDA(cudaMemcpyAsync(ctx->h_flags, d_bad, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     B200_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -532,6 +658,16 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
   return B200_OK;
 }
 
+// the operator's row-offset array of width P (csr.cuh)
+inline int *&rowptr_slot(b200_csr *A, int *) { return A->rowptr; }
+inline int64_t *&rowptr_slot(b200_csr *A, int64_t *) { return A->rowptr64; }
+
+// 8-byte row offsets: single-GPU operators of INT32_MAX or more nonzeros, or every single-GPU operator when the
+// context's "rowptr64" is 1
+bool wants_rowptr64(const b200_ctx *ctx, int64_t nnz) {
+  return ctx->world == 1 && (ctx->opt_rowptr64 == 1 || nnz >= (int64_t)INT32_MAX);
+}
+
 int check_dist_args(b200_ctx *ctx, int64_t n_global, int64_t row_begin, int64_t m_local, const b200_halo_plan *plan) {
   B200_REQUIRE(ctx, "ctx is NULL");
   B200_REQUIRE(m_local >= 0 && row_begin >= 0 && row_begin + m_local <= n_global, "bad slab");
@@ -553,18 +689,26 @@ int check_dist_args(b200_ctx *ctx, int64_t n_global, int64_t row_begin, int64_t 
 // ------------------------------------------------------------------------------------------
 // C ABI: operator construction
 // ------------------------------------------------------------------------------------------
-template <typename I, typename TI, typename T>
-static int csr_from_csc_impl(b200_ctx *ctx, int64_t m, int64_t n, const I *colptr, const I *rowval, const TI *nzval,
+// P: the row offsets built (int, or int64_t: then the permutation is int64_t too and cub counts items in int64_t);
+// IC, IR: the CSC's colptr and rowval (int32_t or int64_t; the adjoint of an 8-byte operator has int64 colptr and
+// int32 rowval).
+template <typename P, typename IC, typename IR, typename TI, typename T>
+static int csr_from_csc_impl(b200_ctx *ctx, int64_t m, int64_t n, const IC *colptr, const IR *rowval, const TI *nzval,
                              int base, int64_t nnz, cudaMemcpyKind src_kind, b200_csr *A) {
   // colptr/rowval/nzval: host arrays (src_kind = cudaMemcpyHostToDevice; nnz = colptr[n] - base read by the caller)
   // or device arrays (cudaMemcpyDeviceToDevice: b200_csr_transpose feeds the CSR arrays of A as the CSC of A')
+  typedef typename std::conditional<sizeof(P) == 8, int64_t, int>::type N;   // cub's num_items
   cudaStream_t st = ctx->stream;
-  B200_REQUIRE(nnz >= 0 && nnz < (int64_t)INT32_MAX, "nnz=%lld does not fit int32 CSR", (long long)nnz);
+  if (sizeof(P) == 4) B200_REQUIRE(nnz >= 0 && nnz < (int64_t)INT32_MAX, "nnz=%lld does not fit int32 CSR", (long long)nnz);
+  B200_REQUIRE(nnz >= 0, "nnz=%lld", (long long)nnz);
   A->nnz = nnz;
-  I *d_colptr = nullptr, *d_rowval = nullptr;
+  IC *d_colptr = nullptr;
+  IR *d_rowval = nullptr;
   TI *d_nz = nullptr;
   unsigned int *key_in = nullptr, *key_out = nullptr;
-  int *col_of = nullptr, *perm_in = nullptr, *perm_out = nullptr, *d_err = nullptr;
+  int *col_of = nullptr, *d_err = nullptr;
+  P *perm_in = nullptr, *perm_out = nullptr;
+  P *&rowptr = rowptr_slot(A, (P *)nullptr);
   void *d_tmp = nullptr;
   size_t tmp_bytes = 0, tmp2 = 0;
   int status = B200_OK;
@@ -581,24 +725,24 @@ static int csr_from_csc_impl(b200_ctx *ctx, int64_t m, int64_t n, const I *colpt
       return B200_ERR_CUDA;               \
     }                                     \
   } while (0)
-  CK(cudaMalloc(&d_colptr, sizeof(I) * (n + 1)));
-  CK(cudaMalloc(&d_rowval, sizeof(I) * (nnz ? nnz : 1)));
+  CK(cudaMalloc(&d_colptr, sizeof(IC) * (n + 1)));
+  CK(cudaMalloc(&d_rowval, sizeof(IR) * (nnz ? nnz : 1)));
   CK(cudaMalloc(&d_nz, sizeof(TI) * (nnz ? nnz : 1)));
   CK(cudaMalloc(&d_err, sizeof(int)));
   CK(cudaMemsetAsync(d_err, 0, sizeof(int), st));
-  CK(cudaMemcpyAsync(d_colptr, colptr, sizeof(I) * (n + 1), src_kind, st));
-  CK(cudaMemcpyAsync(d_rowval, rowval, sizeof(I) * nnz, src_kind, st));
+  CK(cudaMemcpyAsync(d_colptr, colptr, sizeof(IC) * (n + 1), src_kind, st));
+  CK(cudaMemcpyAsync(d_rowval, rowval, sizeof(IR) * nnz, src_kind, st));
   CK(cudaMemcpyAsync(d_nz, nzval, sizeof(TI) * nnz, src_kind, st));
-  CK(cudaMalloc(&A->rowptr, sizeof(int) * (m + kRowptrPad)));
+  CK(cudaMalloc(&rowptr, sizeof(P) * (m + kRowptrPad)));
   CK(cudaMalloc(&A->colind, sizeof(int) * (nnz + kNnzPad)));
   CK(cudaMalloc(&A->vals, sizeof(T) * (nnz + kNnzPad)));
   // rowptr: histogram of row ids, exclusive scan
-  CK(cudaMemsetAsync(A->rowptr, 0, sizeof(int) * (m + kRowptrPad), st));
+  CK(cudaMemsetAsync(rowptr, 0, sizeof(P) * (m + kRowptrPad), st));
   if (nnz) {
-    k_count_rows<I><<<grid_for(ctx, nnz), 256, 0, st>>>(d_rowval, nnz, base, m, A->rowptr, d_err);
+    k_count_rows<IR><<<grid_for(ctx, nnz), 256, 0, st>>>(d_rowval, nnz, base, m, rowptr, d_err);
     ctx->launches++;
   }
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, A->rowptr, A->rowptr, (int)(m + 1), st));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, rowptr, rowptr, (N)(m + 1), st));
   // stable radix sort of (row key, original position): orders by (row, column) because the CSC
   // arrays are column-major with ascending rows inside a column
   int end_bit = 1;
@@ -606,17 +750,17 @@ static int csr_from_csc_impl(b200_ctx *ctx, int64_t m, int64_t n, const I *colpt
   CK(cudaMalloc(&key_in, sizeof(unsigned int) * (nnz ? nnz : 1)));
   CK(cudaMalloc(&key_out, sizeof(unsigned int) * (nnz ? nnz : 1)));
   CK(cudaMalloc(&col_of, sizeof(int) * (nnz + kNnzPad)));
-  CK(cudaMalloc(&perm_in, sizeof(int) * (nnz + kNnzPad)));
-  CK(cudaMalloc(&perm_out, sizeof(int) * (nnz + kNnzPad)));
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp2, key_in, key_out, perm_in, perm_out, (int)nnz, 0, end_bit, st));
+  CK(cudaMalloc(&perm_in, sizeof(P) * (nnz + kNnzPad)));
+  CK(cudaMalloc(&perm_out, sizeof(P) * (nnz + kNnzPad)));
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp2, key_in, key_out, perm_in, perm_out, (N)nnz, 0, end_bit, st));
   tmp_bytes = std::max(tmp_bytes, tmp2);
   CK(cudaMalloc(&d_tmp, tmp_bytes ? tmp_bytes : 16));
-  CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, A->rowptr, A->rowptr, (int)(m + 1), st));
+  CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, rowptr, rowptr, (N)(m + 1), st));
   ctx->launches++;
   if (nnz) {
-    k_expand_cols<I><<<grid_for(ctx, n * 32), 256, 0, st>>>(d_colptr, n, base, d_rowval, key_in, col_of);
+    k_expand_cols<<<grid_for(ctx, n * 32), 256, 0, st>>>(d_colptr, n, base, d_rowval, key_in, col_of);
     k_iota<<<grid_for(ctx, nnz), 256, 0, st>>>(perm_in, nnz);
-    CK(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, key_in, key_out, perm_in, perm_out, (int)nnz, 0, end_bit, st));
+    CK(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, key_in, key_out, perm_in, perm_out, (N)nnz, 0, end_bit, st));
     k_gather_int<<<grid_for(ctx, nnz), 256, 0, st>>>(perm_out, col_of, nnz, A->colind);
     k_gather_vals<T, TI><<<grid_for(ctx, nnz), 256, 0, st>>>(perm_out, d_nz, nnz, (T *)A->vals);
     ctx->launches += 5;
@@ -650,23 +794,24 @@ int b200_csr_from_csc(b200_ctx *ctx, int64_t m, int64_t n, const void *colptr, c
   A->m_global = m;
   A->n_global = n;
   const int64_t nnz = (idx_bytes == 8 ? (int64_t)((const int64_t *)colptr)[n] : (int64_t)((const int32_t *)colptr)[n]) - base;
-  const cudaMemcpyKind h2d = cudaMemcpyHostToDevice;
-  int s;
-  if (is_complex_dtype(dtype)) {
-    // the same upload / sort / gather pipeline with a 16-byte (ComplexF64) or 8-byte (ComplexF32) value type
-    if (idx_bytes == 8)
-      s = dtype == B200_CF64 ? csr_from_csc_impl<int64_t, cplx<double>, cplx<double>>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const cplx<double> *)nzval, base, nnz, h2d, A)
-                             : csr_from_csc_impl<int64_t, cplx<float>, cplx<float>>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const cplx<float> *)nzval, base, nnz, h2d, A);
-    else
-      s = dtype == B200_CF64 ? csr_from_csc_impl<int32_t, cplx<double>, cplx<double>>(ctx, m, n, (const int32_t *)colptr, (const int32_t *)rowval, (const cplx<double> *)nzval, base, nnz, h2d, A)
-                             : csr_from_csc_impl<int32_t, cplx<float>, cplx<float>>(ctx, m, n, (const int32_t *)colptr, (const int32_t *)rowval, (const cplx<float> *)nzval, base, nnz, h2d, A);
-  } else if (idx_bytes == 8) {
-    s = dtype == B200_F64 ? csr_from_csc_impl<int64_t, double, double>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const double *)nzval, base, nnz, h2d, A)
-                          : csr_from_csc_impl<int64_t, float, float>(ctx, m, n, (const int64_t *)colptr, (const int64_t *)rowval, (const float *)nzval, base, nnz, h2d, A);
-  } else {
-    s = dtype == B200_F64 ? csr_from_csc_impl<int32_t, double, double>(ctx, m, n, (const int32_t *)colptr, (const int32_t *)rowval, (const double *)nzval, base, nnz, h2d, A)
-                          : csr_from_csc_impl<int32_t, float, float>(ctx, m, n, (const int32_t *)colptr, (const int32_t *)rowval, (const float *)nzval, base, nnz, h2d, A);
-  }
+  // the upload / sort / gather pipeline at the index width of the arrays, the element type and the row-offset width
+  auto conv = [&](auto idx, auto elt) -> int {
+    typedef decltype(idx) I;
+    typedef decltype(elt) T;
+    const I *cp = (const I *)colptr, *rv = (const I *)rowval;
+    if (wants_rowptr64(ctx, nnz))
+      return csr_from_csc_impl<int64_t, I, I, T, T>(ctx, m, n, cp, rv, (const T *)nzval, base, nnz, cudaMemcpyHostToDevice, A);
+    return csr_from_csc_impl<int, I, I, T, T>(ctx, m, n, cp, rv, (const T *)nzval, base, nnz, cudaMemcpyHostToDevice, A);
+  };
+  auto by_dtype = [&](auto idx) -> int {
+    switch (dtype) {
+      case B200_F64: return conv(idx, double());
+      case B200_F32: return conv(idx, float());
+      case B200_CF64: return conv(idx, cplx<double>());
+      default: return conv(idx, cplx<float>());
+    }
+  };
+  int s = idx_bytes == 8 ? by_dtype(int64_t()) : by_dtype(int32_t());
   if (s == B200_OK) s = finish_operator(ctx, A, nullptr);
   if (s != B200_OK) {
     b200_csr_destroy(A);
@@ -693,11 +838,15 @@ int b200_csr_transpose(b200_ctx *ctx, const b200_csr *A, b200_csr **out) {
   At->m_global = A->n_global;
   At->n_global = A->m_local;
   const cudaMemcpyKind d2d = cudaMemcpyDeviceToDevice;
-  int s = A->dtype == B200_F64
-              ? csr_from_csc_impl<int32_t, double, double>(ctx, At->m_local, At->n_global, A->rowptr, A->colind,
-                                                           (const double *)A->vals, 0, A->nnz, d2d, At)
-              : csr_from_csc_impl<int32_t, float, float>(ctx, At->m_local, At->n_global, A->rowptr, A->colind,
-                                                         (const float *)A->vals, 0, A->nnz, d2d, At);
+  // the adjoint keeps A's row-offset width (A's offsets are the colptr of the CSC of A')
+  int s = with_rowptr(A, [&](auto rp) -> int {
+    typedef typename std::remove_const<typename std::remove_pointer<decltype(rp)>::type>::type P;
+    return A->dtype == B200_F64
+               ? csr_from_csc_impl<P, P, int, double, double>(ctx, At->m_local, At->n_global, rp, A->colind,
+                                                              (const double *)A->vals, 0, A->nnz, d2d, At)
+               : csr_from_csc_impl<P, P, int, float, float>(ctx, At->m_local, At->n_global, rp, A->colind,
+                                                            (const float *)A->vals, 0, A->nnz, d2d, At);
+  });
   if (s == B200_OK) s = finish_operator(ctx, At, nullptr);
   if (s != B200_OK) {
     b200_csr_destroy(At);
@@ -718,7 +867,8 @@ int b200_csr_from_csr_slab(b200_ctx *ctx, int64_t n_global, int64_t row_begin, i
   cudaStream_t st = ctx->stream;
   const int64_t nnz = idx_bytes == 8 ? ((const int64_t *)rowptr)[m_local] - ((const int64_t *)rowptr)[0]
                                      : (int64_t)((const int32_t *)rowptr)[m_local] - ((const int32_t *)rowptr)[0];
-  B200_REQUIRE(nnz >= 0 && nnz < (int64_t)INT32_MAX, "local nnz must fit int32");
+  const bool wide = wants_rowptr64(ctx, nnz);   // multi-GPU slabs keep int32 row offsets
+  B200_REQUIRE(nnz >= 0 && (wide || nnz < (int64_t)INT32_MAX), "local nnz must fit int32");
   auto *A = new b200_csr();
   A->ctx = ctx;
   A->dtype = dtype;
@@ -746,8 +896,13 @@ int b200_csr_from_csr_slab(b200_ctx *ctx, int64_t n_global, int64_t row_begin, i
       return fail(B200_ERR_CUDA);                                                       \
     }                                                                                   \
   } while (0)
-  CK(cudaMalloc(&A->rowptr, sizeof(int) * (m_local + kRowptrPad)));
-  CK(cudaMemsetAsync(A->rowptr, 0, sizeof(int) * (m_local + kRowptrPad), st));
+  if (wide) {
+    CK(cudaMalloc(&A->rowptr64, sizeof(int64_t) * (m_local + kRowptrPad)));
+    CK(cudaMemsetAsync(A->rowptr64, 0, sizeof(int64_t) * (m_local + kRowptrPad), st));
+  } else {
+    CK(cudaMalloc(&A->rowptr, sizeof(int) * (m_local + kRowptrPad)));
+    CK(cudaMemsetAsync(A->rowptr, 0, sizeof(int) * (m_local + kRowptrPad), st));
+  }
   CK(cudaMalloc(&A->colind, sizeof(int) * (nnz + kNnzPad)));
   CK(cudaMalloc(&A->vals, vs * (nnz + kNnzPad)));
   CK(cudaMalloc(&d_rp, (size_t)idx_bytes * (m_local + 1)));
@@ -764,10 +919,12 @@ int b200_csr_from_csr_slab(b200_ctx *ctx, int64_t n_global, int64_t row_begin, i
     CK(cudaMemcpyAsync(d_halo, plan->halo_sorted.data(), sizeof(int64_t) * A->n_halo, cudaMemcpyHostToDevice, st));
   const int64_t lo = row_begin, hi = row_begin + m_local;
   if (idx_bytes == 8) {
-    k_rowptr_convert<int64_t><<<grid_for(ctx, m_local + 1), 256, 0, st>>>((const int64_t *)d_rp, m_local, A->rowptr);
+    if (wide) k_rowptr_convert<int64_t><<<grid_for(ctx, m_local + 1), 256, 0, st>>>((const int64_t *)d_rp, m_local, A->rowptr64);
+    else k_rowptr_convert<int64_t><<<grid_for(ctx, m_local + 1), 256, 0, st>>>((const int64_t *)d_rp, m_local, A->rowptr);
     if (nnz) k_remap_cols<int64_t><<<grid_for(ctx, nnz), 256, 0, st>>>((const int64_t *)d_ci, nnz, base, lo, hi, d_halo, A->n_halo, A->colind, d_err);
   } else {
-    k_rowptr_convert<int32_t><<<grid_for(ctx, m_local + 1), 256, 0, st>>>((const int32_t *)d_rp, m_local, A->rowptr);
+    if (wide) k_rowptr_convert<int32_t><<<grid_for(ctx, m_local + 1), 256, 0, st>>>((const int32_t *)d_rp, m_local, A->rowptr64);
+    else k_rowptr_convert<int32_t><<<grid_for(ctx, m_local + 1), 256, 0, st>>>((const int32_t *)d_rp, m_local, A->rowptr);
     if (nnz) k_remap_cols<int32_t><<<grid_for(ctx, nnz), 256, 0, st>>>((const int32_t *)d_ci, nnz, base, lo, hi, d_halo, A->n_halo, A->colind, d_err);
   }
   ctx->launches += 2;
@@ -813,6 +970,11 @@ int b200_csr_laplacian(b200_ctx *ctx, int64_t N, int dims, int dtype, int64_t ro
   A->n_global = n;
   A->row_begin = row_begin;
   A->n_halo = plan ? (int64_t)plan->halo_sorted.size() : 0;
+  // nnz of the whole operator: n diagonal entries and 2 (N-1) N^(dims-1) off-diagonal ones per dimension; only a
+  // single-GPU operator (all rows) can take 8-byte row offsets
+  int64_t nnz_all = n;
+  for (int d = 0; d < dims; ++d) nnz_all += 2 * (N - 1) * (n / N);
+  const bool wide = wants_rowptr64(ctx, nnz_all);
   int64_t *d_halo = nullptr;
   void *d_tmp = nullptr;
   size_t tmp_bytes = 0;
@@ -829,28 +991,37 @@ int b200_csr_laplacian(b200_ctx *ctx, int64_t N, int dims, int dtype, int64_t ro
       return fail(B200_ERR_CUDA);                                                       \
     }                                                                                   \
   } while (0)
-  CK(cudaMalloc(&A->rowptr, sizeof(int) * (m_local + kRowptrPad)));
-  CK(cudaMemsetAsync(A->rowptr, 0, sizeof(int) * (m_local + kRowptrPad), st));
   CK(cudaMalloc(&d_halo, sizeof(int64_t) * (A->n_halo ? A->n_halo : 1)));
   if (A->n_halo)
     CK(cudaMemcpyAsync(d_halo, plan->halo_sorted.data(), sizeof(int64_t) * A->n_halo, cudaMemcpyHostToDevice, st));
-  if (m_local) k_lap_count<<<grid_for(ctx, m_local), 256, 0, st>>>(g, row_begin, m_local, A->rowptr);
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, A->rowptr, A->rowptr, (int)(m_local + 1), st));
-  CK(cudaMalloc(&d_tmp, tmp_bytes ? tmp_bytes : 16));
-  CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, A->rowptr, A->rowptr, (int)(m_local + 1), st));
-  int nnz32 = 0;
-  CK(cudaMemcpyAsync(&nnz32, A->rowptr + m_local, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  A->nnz = nnz32;
-  const size_t vs = dtype_size(dtype);
-  CK(cudaMalloc(&A->colind, sizeof(int) * (A->nnz + kNnzPad)));
-  CK(cudaMalloc(&A->vals, vs * (A->nnz + kNnzPad)));
-  if (m_local) {
-    if (dtype == B200_F64)
-      k_lap_fill<double><<<grid_for(ctx, m_local), 256, 0, st>>>(g, row_begin, m_local, A->rowptr, d_halo, A->n_halo, A->colind, (double *)A->vals);
-    else
-      k_lap_fill<float><<<grid_for(ctx, m_local), 256, 0, st>>>(g, row_begin, m_local, A->rowptr, d_halo, A->n_halo, A->colind, (float *)A->vals);
-  }
+  // counts, exclusive scan, fill through the offsets, at the operator's row-offset width P
+  auto build = [&](auto *rp) -> int {
+    typedef typename std::remove_pointer<decltype(rp)>::type P;
+    typedef typename std::conditional<sizeof(P) == 8, int64_t, int>::type NI;   // cub's num_items
+    P *&rowptr = rowptr_slot(A, rp);
+    CK(cudaMalloc(&rowptr, sizeof(P) * (m_local + kRowptrPad)));
+    CK(cudaMemsetAsync(rowptr, 0, sizeof(P) * (m_local + kRowptrPad), st));
+    if (m_local) k_lap_count<<<grid_for(ctx, m_local), 256, 0, st>>>(g, row_begin, m_local, rowptr);
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, rowptr, rowptr, (NI)(m_local + 1), st));
+    CK(cudaMalloc(&d_tmp, tmp_bytes ? tmp_bytes : 16));
+    CK(cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, rowptr, rowptr, (NI)(m_local + 1), st));
+    P nnz_local = 0;
+    CK(cudaMemcpyAsync(&nnz_local, rowptr + m_local, sizeof(P), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    A->nnz = nnz_local;
+    const size_t vs = dtype_size(dtype);
+    CK(cudaMalloc(&A->colind, sizeof(int) * (A->nnz + kNnzPad)));
+    CK(cudaMalloc(&A->vals, vs * (A->nnz + kNnzPad)));
+    if (m_local) {
+      if (dtype == B200_F64)
+        k_lap_fill<double><<<grid_for(ctx, m_local), 256, 0, st>>>(g, row_begin, m_local, rowptr, d_halo, A->n_halo, A->colind, (double *)A->vals);
+      else
+        k_lap_fill<float><<<grid_for(ctx, m_local), 256, 0, st>>>(g, row_begin, m_local, rowptr, d_halo, A->n_halo, A->colind, (float *)A->vals);
+    }
+    return B200_OK;
+  };
+  if (wide) B200_TRY(build((int64_t *)nullptr));
+  else B200_TRY(build((int *)nullptr));
   ctx->launches += 3;
   CK(cudaStreamSynchronize(st));
   CK(cudaGetLastError());
@@ -872,6 +1043,7 @@ int b200_csr_destroy(b200_csr *A) {
     cudaStreamSynchronize(A->ctx->stream);
   }
   cudaFree(A->rowptr);
+  cudaFree(A->rowptr64);
   cudaFree(A->colind);
   cudaFree(A->vals);
   cudaFree(A->send_idx);
@@ -906,7 +1078,7 @@ int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes)
     bytes = ntiles * (int64_t)(sizeof(b200_band_tile) + kBandTileRows);
   } else {
     k = A->stream_lpr > 0 ? 2 : 1;
-    bytes = 4 * A->nnz + 4 * (A->m_local + 1);
+    bytes = 4 * A->nnz + (A->rowptr64 ? 8 : 4) * (A->m_local + 1);
   }
   if (kind) *kind = k;
   if (structure_bytes) *structure_bytes = bytes;
@@ -916,24 +1088,55 @@ int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes)
 int b200_csr_diag(b200_ctx *ctx, const b200_csr *A, void *diag_dev) {
   B200_REQUIRE(ctx && A && diag_dev, "NULL argument");
   if (A->m_local == 0) return B200_OK;
-  if (A->dtype == B200_CF64)
-    k_diag<cplx<double>><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const cplx<double> *)A->vals, A->m_local, (cplx<double> *)diag_dev);
-  else if (A->dtype == B200_CF32)
-    k_diag<cplx<float>><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const cplx<float> *)A->vals, A->m_local, (cplx<float> *)diag_dev);
-  else if (A->dtype == B200_F64)
-    k_diag<double><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const double *)A->vals, A->m_local, (double *)diag_dev);
-  else
-    k_diag<float><<<grid_for(ctx, A->m_local), 256, 0, ctx->stream>>>(A->rowptr, A->colind, (const float *)A->vals, A->m_local, (float *)diag_dev);
+  const int grid = grid_for(ctx, A->m_local);
+  with_rowptr(A, [&](auto rp) {
+    if (A->dtype == B200_CF64)
+      k_diag<cplx<double>><<<grid, 256, 0, ctx->stream>>>(rp, A->colind, (const cplx<double> *)A->vals, A->m_local, (cplx<double> *)diag_dev);
+    else if (A->dtype == B200_CF32)
+      k_diag<cplx<float>><<<grid, 256, 0, ctx->stream>>>(rp, A->colind, (const cplx<float> *)A->vals, A->m_local, (cplx<float> *)diag_dev);
+    else if (A->dtype == B200_F64)
+      k_diag<double><<<grid, 256, 0, ctx->stream>>>(rp, A->colind, (const double *)A->vals, A->m_local, (double *)diag_dev);
+    else
+      k_diag<float><<<grid, 256, 0, ctx->stream>>>(rp, A->colind, (const float *)A->vals, A->m_local, (float *)diag_dev);
+    return 0;
+  });
   B200_LAUNCH_CHECK(ctx);
   return B200_OK;
 }
 
 int b200_csr_download(b200_ctx *ctx, const b200_csr *A, int32_t *rowptr, int32_t *colind, void *vals) {
   B200_REQUIRE(ctx && A, "NULL argument");
+  if (A->rowptr64) {
+    set_error("b200_csr_download: the operator has 8-byte row offsets (nnz >= 2^31, or built with \"rowptr64\" = 1); "
+              "use b200_csr_download64");
+    return B200_ERR_UNSUPPORTED;
+  }
   if (rowptr) B200_CUDA(cudaMemcpyAsync(rowptr, A->rowptr, sizeof(int) * (A->m_local + 1), cudaMemcpyDeviceToHost, ctx->stream));
   if (colind && A->nnz) B200_CUDA(cudaMemcpyAsync(colind, A->colind, sizeof(int) * A->nnz, cudaMemcpyDeviceToHost, ctx->stream));
   if (vals && A->nnz) B200_CUDA(cudaMemcpyAsync(vals, A->vals, dtype_size(A->dtype) * A->nnz, cudaMemcpyDeviceToHost, ctx->stream));
   B200_CUDA(cudaStreamSynchronize(ctx->stream));
+  return B200_OK;
+}
+
+int b200_csr_download64(b200_ctx *ctx, const b200_csr *A, int64_t *rowptr, int32_t *colind, void *vals) {
+  B200_REQUIRE(ctx && A, "NULL argument");
+  std::vector<int> narrow;
+  if (rowptr && A->rowptr64) {
+    B200_CUDA(cudaMemcpyAsync(rowptr, A->rowptr64, sizeof(int64_t) * (A->m_local + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  } else if (rowptr) {
+    narrow.resize((size_t)A->m_local + 1);
+    B200_CUDA(cudaMemcpyAsync(narrow.data(), A->rowptr, sizeof(int) * (A->m_local + 1), cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (colind && A->nnz) B200_CUDA(cudaMemcpyAsync(colind, A->colind, sizeof(int) * A->nnz, cudaMemcpyDeviceToHost, ctx->stream));
+  if (vals && A->nnz) B200_CUDA(cudaMemcpyAsync(vals, A->vals, dtype_size(A->dtype) * A->nnz, cudaMemcpyDeviceToHost, ctx->stream));
+  B200_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (size_t i = 0; i < narrow.size(); ++i) rowptr[i] = narrow[i];
+  return B200_OK;
+}
+
+int b200_csr_index_bytes(const b200_csr *A, int *bytes) {
+  B200_REQUIRE(A && bytes, "NULL argument");
+  *bytes = A->rowptr64 ? 8 : 4;
   return B200_OK;
 }
 

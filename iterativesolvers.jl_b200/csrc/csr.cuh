@@ -1,4 +1,5 @@
-// csr.cuh -- the device operator (CSR int32, row slab) and the host halo plan.
+// csr.cuh -- the device operator (CSR with int32 column indices and int32 or int64 row offsets, row slab) and the
+// host halo plan.
 #pragma once
 #include "common.cuh"
 
@@ -23,7 +24,9 @@ using b200::kNnzPad;
 using b200::kRowptrPad;
 
 // Per-tile header of the band description.  Tile t covers rows [t*R, min(t*R+R, m)), R = kBandTileRows; its nonzeros are
-// vals[k0, k1) (= rowptr[r0], rowptr[r1]) in row order, and within a row in ascending offset order.
+// vals[k0, k1) (= rowptr[r0], rowptr[r1]) in row order, and within a row in ascending offset order.  Operators with
+// 8-byte row offsets store the low 32 bits of both bounds in k0, k1 and the high 32 bits of the first in pad[0]: a tile
+// holds fewer than 2^32 nonzeros, so k1 = k0 + (uint32_t)(k1_lo - k0_lo).  pad[0] is 0 for 4-byte operators.
 struct alignas(16) b200_band_tile {
   int off[8];   // the tile's distinct offsets col - row, ascending; entries >= nb are 0
   int nb;       // number of offsets
@@ -38,7 +41,10 @@ struct b200_csr {
   int dtype = B200_F64;
   int64_t m_local = 0, n_global = 0, row_begin = 0, nnz = 0, n_halo = 0;
   int64_t m_global = 0;    // size(A,1); != n_global only for single-GPU rectangular operators (lsqr!/lsmr!)
-  int *rowptr = nullptr;   // m_local+1
+  // row offsets, m_local+1 (+ kRowptrPad): exactly one of the two is allocated.  Single-GPU operators with nnz >=
+  // INT32_MAX (or built on a context with "rowptr64" = 1) get rowptr64, every other operator rowptr.
+  int *rowptr = nullptr;
+  int64_t *rowptr64 = nullptr;
   int *colind = nullptr;   // nnz; local extended index: [0,m_local) own, [m_local,m_local+n_halo) halo
   void *vals = nullptr;    // nnz
   int max_row_nnz = 0;
@@ -75,6 +81,11 @@ int halo_exchange(b200_ctx *ctx, const b200_csr *A, const void *x_dev);
 // (skipped on the device when *done_flag != 0); consumers wait with peer_wait_halo(.., A->recv_mask, seq)
 int halo_push(b200_ctx *ctx, const b200_csr *A, const void *x_dev, unsigned long long seq, const int *done_flag);
 inline bool is_square(const b200_csr *A) { return A->m_global == A->n_global; }
+// f(rowptr) with the operator's row offsets at their own width (const int * or const int64_t *)
+template <typename F>
+inline auto with_rowptr(const b200_csr *A, F &&f) {
+  return A->rowptr64 ? f((const int64_t *)A->rowptr64) : f((const int *)A->rowptr);
+}
 // real_only (common.cuh) for an operator argument (NULL is left to the entry point's own argument check)
 inline int real_only(const b200_csr *A, const char *entry) { return A ? real_only(A->dtype, entry) : B200_OK; }
 inline bool use_peer(const b200_ctx *ctx, const b200_csr *A) {

@@ -253,6 +253,11 @@ int b200_ctx_set_option(b200_ctx *c, const char *name, int64_t value) {
     c->opt_cg_persistent = value != 0;
     return B200_OK;
   }
+  if (strcmp(name, "rowptr64") == 0) {
+    B200_REQUIRE(value == 0 || value == 1, "rowptr64 must be 0 (automatic) or 1 (always 8-byte row offsets)");
+    c->opt_rowptr64 = (int)value;
+    return B200_OK;
+  }
   if (strcmp(name, "fold_push") == 0) {
     c->opt_fold_push = value != 0;
     return B200_OK;
@@ -289,6 +294,7 @@ int b200_ctx_get_option(const b200_ctx *c, const char *name, int64_t *value) {
   else if (strcmp(name, "pdl") == 0) *value = c->opt_pdl;
   else if (strcmp(name, "fold_push") == 0) *value = c->opt_fold_push;
   else if (strcmp(name, "cg_persistent") == 0) *value = c->opt_cg_persistent;
+  else if (strcmp(name, "rowptr64") == 0) *value = c->opt_rowptr64;
   else if (strcmp(name, "peer_ok") == 0) *value = c->peer_ok ? 1 : 0;
   else {
     set_error("unknown option `%s`", name);

@@ -131,27 +131,28 @@ __global__ void __launch_bounds__(kThreads) k_pack_rows(const int *__restrict__ 
 
 // Y = A X on row-major blocks: 4 lanes per row, each lane owns 4 of the 16 columns, so every nonzero is one
 // coalesced 64-byte (fp32) read of the X row.
-template <typename T>
-__global__ void __launch_bounds__(kThreads) k_spmm_rm(const int *__restrict__ rowptr, const int *__restrict__ colind,
-                                                      const T *__restrict__ vals, const T *__restrict__ X,
-                                                      const T *__restrict__ Xhalo, int64_t m, T *__restrict__ Y) {
+// k_spmm_rm has an overload per row-offset width (int, int64_t; spmv_launch.cuh says why overloads).
+template <typename T, typename I>
+__device__ __forceinline__ void spmm_rm_rows(const I *__restrict__ rowptr, const int *__restrict__ colind,
+                                             const T *__restrict__ vals, const T *__restrict__ X,
+                                             const T *__restrict__ Xhalo, int64_t m, T *__restrict__ Y) {
   const int sub = threadIdx.x & 3;
   const int rib = threadIdx.x >> 2;
   const uint64_t pol = policy_evict_first();
   for (int64_t base = (int64_t)blockIdx.x * (kThreads / 4); base < m; base += (int64_t)gridDim.x * (kThreads / 4)) {
     const int64_t row = base + rib;
     if (row >= m) continue;
-    const int b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
+    const I b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
     T acc[4] = {(T)0, (T)0, (T)0, (T)0};
     // four nonzeros per round: their column indices, then their four X rows are in flight together (the one-by-one loop
     // chains index load -> gather -> FMA per nonzero and is latency-bound); the products are added
     // in the row's storage order, as before
-    for (int k = b; k < e; k += 4) {
+    for (I k = b; k < e; k += 4) {
       int c[4];
       T a[4];
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
-        const int kk = k + u < e ? k + u : e - 1;
+        const I kk = k + u < e ? k + u : e - 1;
         c[u] = ld_stream<int>(colind + kk, pol);
         a[u] = ld_stream<T>(vals + kk, pol);
         if (k + u >= e) a[u] = (T)0;
@@ -185,6 +186,18 @@ __global__ void __launch_bounds__(kThreads) k_spmm_rm(const int *__restrict__ ro
       reinterpret_cast<double2 *>(yr)[1] = make_double2(acc[2], acc[3]);
     }
   }
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_spmm_rm(const int *__restrict__ rowptr, const int *__restrict__ colind,
+                                                      const T *__restrict__ vals, const T *__restrict__ X,
+                                                      const T *__restrict__ Xhalo, int64_t m, T *__restrict__ Y) {
+  spmm_rm_rows(rowptr, colind, vals, X, Xhalo, m, Y);
+}
+template <typename T>
+__global__ void __launch_bounds__(kThreads) k_spmm_rm(const int64_t *__restrict__ rowptr, const int *__restrict__ colind,
+                                                      const T *__restrict__ vals, const T *__restrict__ X,
+                                                      const T *__restrict__ Xhalo, int64_t m, T *__restrict__ Y) {
+  spmm_rm_rows(rowptr, colind, vals, X, Xhalo, m, Y);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1099,8 +1112,11 @@ struct Lobpcg {
   int spmm(const T *Xin, T *Yout) {
     B200_TRY(halo_block(Xin));
     ProfScope prof(ctx, 0);
-    k_spmm_rm<T><<<grid_spmm, kThreads, 0, ctx->stream>>>(A->rowptr, A->colind, (const T *)A->vals, Xin,
-                                                          (const T *)halo_blk.p, n, Yout);
+    with_rowptr(A, [&](auto rowptr) {
+      k_spmm_rm<T><<<grid_spmm, kThreads, 0, ctx->stream>>>(rowptr, A->colind, (const T *)A->vals, Xin,
+                                                            (const T *)halo_blk.p, n, Yout);
+      return 0;
+    });
     B200_LAUNCH_CHECK(ctx);
     return B200_OK;
   }

@@ -24,11 +24,12 @@ struct StoreEpi {
 
 // Y = A X for a column-major block of BS vectors: each sub-warp handles one row and keeps BS
 // accumulators, so A is streamed ONCE for the whole block (the CPU reference re-streams it per column).
-template <typename T, int LPR, int BS>
-__global__ void __launch_bounds__(kThreads) k_spmm(const int *__restrict__ rowptr, const int *__restrict__ colind,
-                                                   const T *__restrict__ vals, const T *__restrict__ X, int64_t ldx,
-                                                   const T *__restrict__ halo, int64_t ldh, int m_own, int64_t m,
-                                                   T *__restrict__ Y, int64_t ldy) {
+// k_spmm has an overload per row-offset width (int, int64_t; spmv_launch.cuh says why overloads).
+template <typename T, int LPR, int BS, typename I>
+__device__ __forceinline__ void spmm_rows(const I *__restrict__ rowptr, const int *__restrict__ colind,
+                                          const T *__restrict__ vals, const T *__restrict__ X, int64_t ldx,
+                                          const T *__restrict__ halo, int64_t ldh, int m_own, int64_t m,
+                                          T *__restrict__ Y, int64_t ldy) {
   constexpr int ROWS = kThreads / LPR;
   const int sub = threadIdx.x % LPR;
   const int rib = threadIdx.x / LPR;
@@ -36,12 +37,12 @@ __global__ void __launch_bounds__(kThreads) k_spmm(const int *__restrict__ rowpt
     const int64_t row = base + rib;
     const bool valid = row < m;
     const int64_t r = valid ? row : (m - 1);
-    const int b = __ldg(rowptr + r), e = __ldg(rowptr + r + 1);
+    const I b = __ldg(rowptr + r), e = __ldg(rowptr + r + 1);
     const uint64_t pol = policy_evict_first();
     T acc[BS];
 #pragma unroll
     for (int j = 0; j < BS; ++j) acc[j] = (T)0;
-    for (int k = b + sub; k < e; k += LPR) {
+    for (I k = b + sub; k < e; k += LPR) {
       const int c = ld_stream<int>(colind + k, pol);
       const T a = ld_stream<T>(vals + k, pol);
       const T *src = c < m_own ? X + c : halo + (c - m_own);
@@ -60,6 +61,20 @@ __global__ void __launch_bounds__(kThreads) k_spmm(const int *__restrict__ rowpt
     }
   }
 }
+template <typename T, int LPR, int BS>
+__global__ void __launch_bounds__(kThreads) k_spmm(const int *__restrict__ rowptr, const int *__restrict__ colind,
+                                                   const T *__restrict__ vals, const T *__restrict__ X, int64_t ldx,
+                                                   const T *__restrict__ halo, int64_t ldh, int m_own, int64_t m,
+                                                   T *__restrict__ Y, int64_t ldy) {
+  spmm_rows<T, LPR, BS>(rowptr, colind, vals, X, ldx, halo, ldh, m_own, m, Y, ldy);
+}
+template <typename T, int LPR, int BS>
+__global__ void __launch_bounds__(kThreads) k_spmm(const int64_t *__restrict__ rowptr, const int *__restrict__ colind,
+                                                   const T *__restrict__ vals, const T *__restrict__ X, int64_t ldx,
+                                                   const T *__restrict__ halo, int64_t ldh, int m_own, int64_t m,
+                                                   T *__restrict__ Y, int64_t ldy) {
+  spmm_rows<T, LPR, BS>(rowptr, colind, vals, X, ldx, halo, ldh, m_own, m, Y, ldy);
+}
 
 template <typename T>
 int launch_spmv(b200_ctx *ctx, const b200_csr *A, const void *x, void *y, const int *gate = nullptr, int gate_mask = 0) {
@@ -76,8 +91,11 @@ int launch_spmm_bs(b200_ctx *ctx, const b200_csr *A, const T *X, int64_t ldx, T 
   const T *halo = A->halo ? (const T *)A->halo : X + A->m_local;
   const int64_t ldh = A->halo ? A->n_halo : ldx;
   with_lpr<2>(lpr, [&](auto l) {
-    k_spmm<T, decltype(l)::value, BS><<<grid, kThreads, 0, ctx->stream>>>(
-        A->rowptr, A->colind, (const T *)A->vals, X, ldx, halo, ldh, (int)A->m_local, A->m_local, Y, ldy);
+    with_rowptr(A, [&](auto rowptr) {
+      k_spmm<T, decltype(l)::value, BS><<<grid, kThreads, 0, ctx->stream>>>(
+          rowptr, A->colind, (const T *)A->vals, X, ldx, halo, ldh, (int)A->m_local, A->m_local, Y, ldy);
+      return 0;
+    });
   });
   B200_LAUNCH_CHECK(ctx);
   return B200_OK;

@@ -1,10 +1,10 @@
 // spmv.cuh -- CSR SpMV building blocks shared by the solver kernels.
 //
-// Layout in HBM: rowptr int32 (m+1), colind int32 (nnz, local extended index), vals T (nnz), all
-// contiguous in row order => a contiguous chunk of rows is a contiguous chunk of the colind/vals
-// streams (12 B/nnz in fp64, read exactly once per SpMV); x is gathered through L1/L2.
+// Layout in HBM: rowptr I (m+1; I = int, or int64_t for operators of 2^31 or more nonzeros, csr.cuh), colind int32
+// (nnz, local extended index), vals T (nnz), all contiguous in row order => a contiguous chunk of rows is a contiguous
+// chunk of the colind/vals streams (12 B/nnz in fp64, read exactly once per SpMV); x is gathered through L1/L2.
 //
-// Algorithmic bytes per SpMV (SURVEY.md section 8d): nnz*(V+4) + (m+1)*4 + 2*m*V.
+// Algorithmic bytes per SpMV (SURVEY.md section 8d): nnz*(V+4) + (m+1)*sizeof(I) + 2*m*V.
 #pragma once
 #include <type_traits>
 
@@ -50,13 +50,13 @@ inline XView<T> make_xview(const b200_csr *A, const void *x_dev, bool peer_halo 
 }
 
 // One sub-warp of LPR lanes computes (A x)[row]; result valid in all LPR lanes.
-template <typename T, int LPR, typename XV>
-__device__ __forceinline__ T row_dot(const int *__restrict__ rowptr, const int *__restrict__ colind,
+template <typename T, int LPR, typename XV, typename I>
+__device__ __forceinline__ T row_dot(const I *__restrict__ rowptr, const int *__restrict__ colind,
                                      const T *__restrict__ vals, const XV &xv, int64_t row, int sub) {
-  const int b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
+  const I b = __ldg(rowptr + row), e = __ldg(rowptr + row + 1);
   const uint64_t pol = policy_evict_first();
   T acc = (T)0;
-  for (int k = b + sub; k < e; k += LPR) {
+  for (I k = b + sub; k < e; k += LPR) {
     const int c = ld_stream<int>(colind + k, pol);
     const T a = ld_stream<T>(vals + k, pol);
     acc += a * xv(c);
@@ -71,8 +71,8 @@ constexpr int kRowsThreads = 256;   // block size of the sub-warp form
 // Sub-warp (LPR lanes) per row over all rows; blocks stride the rows in interleaved chunks so that all resident blocks
 // work on neighbouring rows (keeps the x planes of a stencil matrix in L2).  The epilogue contract is the streamed
 // bodies' (spmv_stream.cuh): the lane that owns a row result calls epi.pre(row) and then epi(row, value, pre).
-template <typename T, int LPR, typename XV, typename Epi>
-__device__ __forceinline__ void spmv_rows(const int *__restrict__ rowptr, const int *__restrict__ colind,
+template <typename T, int LPR, typename XV, typename Epi, typename I>
+__device__ __forceinline__ void spmv_rows(const I *__restrict__ rowptr, const int *__restrict__ colind,
                                           const T *__restrict__ vals, const XV &xv, int64_t m, Epi &epi) {
   constexpr int ROWS = kRowsThreads / LPR;
   const int sub = threadIdx.x % LPR;

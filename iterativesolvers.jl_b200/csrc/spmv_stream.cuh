@@ -47,15 +47,17 @@ constexpr int kStreamNnzCap = 4096;                       // nonzeros per tile
 constexpr int kStreamStages = 4;
 constexpr int kStreamCtasPerSm = 1;
 
-template <typename T>
+// I: the operator's row offsets (csr.cuh), staged at their own width.  8-byte offsets add 2 KB per stage: in fp64 a
+// stage is 53,504 B instead of 51,328 B, and the 4 stages still fit the 227 KB of shared memory.
+template <typename T, typename I = int>
 struct alignas(128) StreamStage {
   T val[kStreamNnzCap + 8];
   int col[kStreamNnzCap + 8];
-  int rp[kStreamTileRows + 8];
+  I rp[kStreamTileRows + 8];
 };
-template <typename T>
+template <typename T, typename I = int>
 struct StreamSmem {
-  StreamStage<T> stage[kStreamStages];
+  StreamStage<T, I> stage[kStreamStages];
   alignas(8) unsigned long long full[kStreamStages];
   alignas(8) unsigned long long empty[kStreamStages];
 };
@@ -96,10 +98,10 @@ __device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, u
 
 // Runs over all tiles of this CTA.  `epi(row, value)` is called once per row by the lane that owns
 // the row result.  Must be called by all kStreamThreads threads of the block.
-template <typename T, int LPR, typename XV, typename Epi>
-__device__ __forceinline__ void spmv_stream_tiles(const int *__restrict__ rowptr, const int *__restrict__ colind,
+template <typename T, int LPR, typename XV, typename Epi, typename I>
+__device__ __forceinline__ void spmv_stream_tiles(const I *__restrict__ rowptr, const int *__restrict__ colind,
                                                   const T *__restrict__ vals, const XV &xv, int64_t m, Epi &epi,
-                                                  StreamSmem<T> *sm, bool rev = false) {
+                                                  StreamSmem<T, I> *sm, bool rev = false) {
   constexpr int R = kStreamTileRows / LPR;          // rows per tile
   constexpr int SLOTS = kStreamGroupThreads / LPR;  // row slots per group; each slot owns rows s and s+SLOTS
   const int tid = threadIdx.x;
@@ -122,7 +124,7 @@ __device__ __forceinline__ void spmv_stream_tiles(const int *__restrict__ rowptr
       const uint64_t pol_stream = policy_evict_first();
       int64_t t = blockIdx.x;
       // bounds of the next tile are fetched one iteration ahead (off the critical path)
-      int k0 = 0, k1 = 0;
+      I k0 = 0, k1 = 0;
       if (t < ntiles) {
         const int64_t r0 = phys(t) * R, r1 = (r0 + R < m) ? (r0 + R) : m;
         k0 = __ldg(rowptr + r0);
@@ -133,17 +135,17 @@ __device__ __forceinline__ void spmv_stream_tiles(const int *__restrict__ rowptr
         const uint32_t ph = (uint32_t)((it / kStreamStages) & 1);
         const int64_t r0 = phys(t) * R;
         const int64_t tn = t + gridDim.x;
-        int nk0 = 0, nk1 = 0;
+        I nk0 = 0, nk1 = 0;
         if (tn < ntiles) {
           const int64_t nr0 = phys(tn) * R, nr1 = (nr0 + R < m) ? (nr0 + R) : m;
           nk0 = __ldg(rowptr + nr0);
           nk1 = __ldg(rowptr + nr1);
         }
         mbar_wait(&sm->empty[s], ph ^ 1u);
-        const int k0a = k0 & ~3;
+        const I k0a = k0 & ~(I)3;
         const uint32_t cnt = (uint32_t)(((k1 - k0a) + 3) & ~3);
-        const uint32_t b_val = cnt * (uint32_t)sizeof(T), b_col = cnt * 4u, b_rp = (uint32_t)(R + 4) * 4u;
-        StreamStage<T> *st = &sm->stage[s];
+        const uint32_t b_val = cnt * (uint32_t)sizeof(T), b_col = cnt * 4u, b_rp = (uint32_t)(R + 4) * (uint32_t)sizeof(I);
+        StreamStage<T, I> *st = &sm->stage[s];
         mbar_expect_tx(&sm->full[s], b_val + b_col + b_rp);
         bulk_g2s(st->rp, rowptr + r0, b_rp, &sm->full[s], pol_stream);
         bulk_g2s(st->col, colind + k0a, b_col, &sm->full[s], pol_stream);
@@ -165,16 +167,16 @@ __device__ __forceinline__ void spmv_stream_tiles(const int *__restrict__ rowptr
       const uint32_t ph = (uint32_t)((k / kStreamStages) & 1);
       const int64_t r0 = phys(t) * R;
       mbar_wait(&sm->full[s], ph);
-      const StreamStage<T> *st = &sm->stage[s];
-      const int k0a = st->rp[0] & ~3;
+      const StreamStage<T, I> *st = &sm->stage[s];
+      const I k0a = st->rp[0] & ~(I)3;
       int b[2], e[2];
       bool valid[2];
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         const int rib = slot + q * SLOTS;
         valid[q] = r0 + rib < m;
-        b[q] = valid[q] ? st->rp[rib] - k0a : 0;
-        e[q] = valid[q] ? st->rp[rib + 1] - k0a : 0;
+        b[q] = valid[q] ? (int)(st->rp[rib] - k0a) : 0;   // tile-relative: a tile holds <= kStreamNnzCap nonzeros
+        e[q] = valid[q] ? (int)(st->rp[rib + 1] - k0a) : 0;
       }
       T acc[2] = {(T)0, (T)0};
       // the epilogue's own per-row operand (e.g. MINRES' v_prev[row]) is requested BEFORE the gathers so that its
@@ -292,7 +294,11 @@ struct BandArgs {
   const b200_band_tile *hdr;
   const uint8_t *mask;
 };
-inline BandArgs make_band_args(const b200_csr *A) { return BandArgs{A->band_hdr, A->band_mask}; }
+// the same description of an operator with 8-byte row offsets: tile bounds k0, k1 are 64-bit (b200_band_tile)
+struct BandArgs64 {
+  const b200_band_tile *hdr;
+  const uint8_t *mask;
+};
 
 #ifdef __CUDACC__
 
@@ -313,8 +319,8 @@ __device__ __forceinline__ void bulk_g2s_plain(void *dst_smem, const void *src_g
 }
 
 // Same contract as spmv_stream_tiles (LPR == 1): `x` (nx entries, 16-byte aligned) is the operand, m the rows.
-template <typename T, typename Epi>
-__device__ __forceinline__ void spmv_band_tiles(const BandArgs ba, const T *__restrict__ vals, const T *__restrict__ x,
+template <typename T, typename Epi, typename BA>
+__device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict__ vals, const T *__restrict__ x,
                                                 int64_t nx, int64_t m, Epi &epi, BandSmem<T> *sm, bool rev = false) {
   constexpr int R = kStreamTileRows;
   constexpr int SLOTS = kStreamGroupThreads;
@@ -360,9 +366,19 @@ __device__ __forceinline__ void spmv_band_tiles(const BandArgs ba, const T *__re
           n2 = __ldg(p + 2);
         }
         const int off[kBandMax] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-        const int nb = h2.x, k0 = h2.y, k1 = h2.z;
+        constexpr bool K64 = std::is_same<BA, BandArgs64>::value;
+        typedef typename std::conditional<K64, int64_t, int>::type K;
+        const int nb = h2.x;
+        K k0, k1;
+        if constexpr (K64) {
+          k0 = (int64_t)(((uint64_t)(uint32_t)h2.w << 32) | (uint32_t)h2.y);
+          k1 = k0 + (uint32_t)(h2.z - h2.y);
+        } else {
+          k0 = h2.y;
+          k1 = h2.z;
+        }
         mbar_wait(&sm->empty[s], ph ^ 1u);
-        const int k0a = k0 & ~3;
+        const K k0a = k0 & ~(K)3;
         const uint32_t b_val = (uint32_t)(((k1 - k0a) + 3) & ~3) * (uint32_t)sizeof(T);
         uint32_t total = b_val + (uint32_t)R;
         int64_t bsj[kBandMax];
@@ -387,7 +403,7 @@ __device__ __forceinline__ void spmv_band_tiles(const BandArgs ba, const T *__re
           }
           sm->band[s][j] = e;
         }
-        sm->kofs[s] = k0 - k0a;
+        sm->kofs[s] = (int)(k0 - k0a);
         st_release_shared(&sm->fill[s], it / kBandStages);   // see the consumers' wait
         BandStage<T> *st = &sm->stage[s];
         mbar_expect_tx(&sm->full[s], total);   // releases the ordinary stores above together with the arrival

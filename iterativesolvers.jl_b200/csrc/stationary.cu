@@ -91,6 +91,11 @@ int b200_stationary(b200_ctx *ctx, const b200_csr *A, void *x_dev, const void *b
   B200_REQUIRE(A->ctx == ctx, "operator belongs to another context");
   B200_REQUIRE(ctx->world == 1, "the stationary methods sweep the whole matrix in order: single-GPU contexts only");
   B200_REQUIRE(is_square(A), "this solver needs a square operator");
+  if (A->rowptr64) {
+    set_error("b200_stationary: the sweeps' analysis holds int32 row offsets; an operator with 8-byte row offsets "
+              "(nnz >= 2^31, or built with \"rowptr64\" = 1) is not supported");
+    return B200_ERR_UNSUPPORTED;
+  }
   const int base = method & ~B200_STATIONARY_DENSE_ARITHMETIC;
   B200_REQUIRE(base >= B200_STATIONARY_JACOBI && base <= B200_STATIONARY_SSOR, "unknown stationary method %d", method);
   static_assert(B200_STATIONARY_JACOBI == ST_JACOBI && B200_STATIONARY_GAUSS_SEIDEL == ST_GAUSS_SEIDEL &&

@@ -60,6 +60,15 @@ class Context:
         check(lib().b200_ctx_create_dist(device, rank, world, raw, C.byref(h)))
         return cls(_handle=h)
 
+    def set_option(self, name: str, value: int):
+        """b200_ctx_set_option (include/b200krylov.h lists the options), e.g. set_option("rowptr64", 1)."""
+        check(lib().b200_ctx_set_option(self._h, name.encode(), int(value)))
+
+    def get_option(self, name: str) -> int:
+        v = C.c_int64()
+        check(lib().b200_ctx_get_option(self._h, name.encode(), C.byref(v)))
+        return int(v.value)
+
     def use_stream(self, cuda_stream: int):
         check(lib().b200_ctx_set_stream(self._h, C.c_void_p(cuda_stream)))
 

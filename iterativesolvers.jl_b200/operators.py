@@ -123,8 +123,10 @@ class HaloPlan:
 
 
 class B200CSR:
-    """The operator A on the device (CSR int32, row slab).  Stands where the reference takes a
-    SparseMatrixCSC: `mul!(y, A, x)`, `size(A, d)`, `eltype(A)` (SURVEY.md section 8b)."""
+    """The operator A on the device (CSR with int32 column indices and 4- or 8-byte row offsets, row slab).  Stands
+    where the reference takes a SparseMatrixCSC: `mul!(y, A, x)`, `size(A, d)`, `eltype(A)` (SURVEY.md section 8b).
+    `index_bytes` is the width of the row offsets: 8 for single-GPU operators of 2^31 - 1 or more nonzeros, or when
+    the context's option "rowptr64" was 1 when the operator was built."""
 
     def __init__(self, ctx: Context, handle):
         self.ctx, self._h = ctx, handle
@@ -136,6 +138,9 @@ class B200CSR:
         self.code = dt.value
         # size(A, 1): row-partitioned (multi-GPU) operators are square; single-GPU ones may be rectangular (lsqr!/lsmr!)
         self.m_global = self.m_local if ctx.world == 1 else self.n_global
+        ib = C.c_int()
+        check(lib().b200_csr_index_bytes(handle, C.byref(ib)))
+        self.index_bytes = ib.value
         self._adjoint = None
 
     # --- constructors -----------------------------------------------------------------------
@@ -233,11 +238,12 @@ class B200CSR:
         return d
 
     def download(self):
-        rowptr = np.empty(self.m_local + 1, dtype=np.int32)
+        """(rowptr, colind, vals) of the local rows; rowptr is int32 for 4-byte operators and int64 for 8-byte ones."""
+        rowptr = np.empty(self.m_local + 1, dtype=np.int64)
         colind = np.empty(self.nnz, dtype=np.int32)
         vals = np.empty(self.nnz, dtype=self.dtype)
-        check(lib().b200_csr_download(self.ctx._h, self._h, _vp(rowptr), _vp(colind), _vp(vals)))
-        return rowptr, colind, vals
+        check(lib().b200_csr_download64(self.ctx._h, self._h, _vp(rowptr), _vp(colind), _vp(vals)))
+        return (rowptr if self.index_bytes == 8 else rowptr.astype(np.int32)), colind, vals
 
     def close(self):
         if getattr(self, "_adjoint", None) is not None and getattr(self._adjoint, "_adjoint_of", None) is self:
