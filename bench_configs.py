@@ -23,6 +23,10 @@
     large     (command line only) an operator above 2^31 nonzeros: laplace_matrix(Float64, 680, 3) built on the device
               (2 198 249 600 nonzeros, 8-byte row offsets): cg! it/s and mul!'s ms per launch and GB/s.  Prints a
               "skipped" record instead when the GPU has too little free memory (about 47 GiB are needed)
+    ilu       (command line only) the ILU(0) preconditioner (DESIGN section 22): cg! on laplace_matrix(Float64, N, 3) with
+              Jacobi and with ILU(0); gmres!(30, CGS) and bicgstabl!(2) on advection_dominated(N) with Identity and with
+              ILU(0); each to the default reltol (the unpreconditioned runs capped).  Per record: iterations, time to
+              solution, factorization time, ms per ldiv!, levels per sweep, bytes of each triangular solve, card and power
 
 Each line is a JSON object with iterations/s, per-kernel-class CUDA-event times recorded inside the run
 (b200_ctx_profile_*), the algorithmic bytes (SURVEY.md section 8d) and the achieved fraction of the measured
@@ -534,10 +538,98 @@ def run_large(grid=680, iters=None, reps=2, ctx=None):
     return rec
 
 
+def _ilu_record(isb, ctx, P, n, V=8, applies=20):
+    """ms per ldiv! (CUDA events over `applies` back-to-back applies), levels and algorithmic bytes of each triangular
+    solve.  Forward: L's values and column indices, and per row its row offset, diagonal position, schedule entry and
+    ready flag (16 B), x read, y written, y gathered once; backward: U's strictly upper part likewise plus u_ii."""
+    xd = isb.DeviceArray.from_numpy(ctx, np.random.default_rng(3).standard_normal(n))
+    yd = isb.DeviceArray(ctx, n)
+    P.ldiv_(yd, xd)
+    ctx.sync()
+    ctx.timer_start()
+    for _ in range(applies):
+        P.ldiv_(yd, xd)
+    ms = ctx.timer_stop() / applies
+    fwd_b = P.nnz_lower * (V + 4) + n * (16 + 3 * V)
+    bwd_b = P.nnz_upper * (V + 4) + n * (16 + 4 * V)
+    return {"ldiv_ms": ms, "levels_forward": P.levels[0], "levels_backward": P.levels[1],
+            "forward_solve_bytes": fwd_b, "backward_solve_bytes": bwd_b,
+            "ldiv_gbs_on_algorithmic_bytes": (fwd_b + bwd_b) / (ms * 1e-3) / 1e9}
+
+
+def run_ilu(grid=256, ctx=None, gmres_maxiter=3000, bicgstabl_max_mv=6000):
+    """the `ilu` workloads: cg! (Jacobi vs ILU(0)) on laplace_matrix(Float64, N, 3); gmres!(30) CGS and bicgstabl!(2)
+    (Identity vs ILU(0)) on advection_dominated(N); each to the default reltol, with caps on the unpreconditioned runs"""
+    import iterativesolvers_jl_b200 as isb
+    ctx = ctx or isb.default_context()
+    N = grid
+    n = N ** 3
+    gpu = gpu_name_power(ctx.device)
+    rng = np.random.default_rng(1234321)
+    out = []
+
+    def timed(fn):
+        ctx.sync()
+        t0 = time.perf_counter()
+        r = fn()
+        ctx.sync()
+        return r, time.perf_counter() - t0
+
+    def factor(A):
+        P, dt = timed(lambda: isb.ILU0Prec(A))
+        return P, dt
+
+    A = isb.B200CSR.laplacian(N, 3, np.float64, ctx=ctx)
+    b = rng.standard_normal(n)
+    b /= np.linalg.norm(b)
+    bd = isb.DeviceArray.from_numpy(ctx, b)
+    xd = isb.DeviceArray.zeros(ctx, n)
+    P, t_fact = factor(A)
+    runs = {}
+    for name, Pl in (("jacobi", isb.JacobiPrec(A.diag())), ("ilu0", P)):
+        for rep in range(2):
+            isb.lib().b200_fill(ctx._h, n, 0.0, xd._p, 0)
+            (x, h), dt = timed(lambda: isb.cg_(xd, A, bd, Pl=Pl, initially_zero=True, log=True))
+        runs[name] = {"iters": h.niters, "converged": h.isconverged, "seconds": dt,
+                      "final_resnorm": float(h["resnorm"][-1])}
+    out.append({"config": "ilu", "solver": "cg!, laplace_matrix(Float64, %d, 3), default reltol" % N, "grid": N, "n": n,
+                "nnz": int(A.nnz), **gpu, "runs": runs, "ilu0_factor_seconds": t_fact, **_ilu_record(isb, ctx, P, n),
+                "ilu0_over_jacobi_time": runs["ilu0"]["seconds"] / runs["jacobi"]["seconds"]})
+    P.close()
+    del P, A
+    cp, rv, nz, shape, badv = isb.advection_dominated(N, 1000.0, base=1)
+    A = isb.B200CSR.from_csc_arrays(cp, rv, nz, shape, base=1, ctx=ctx)
+    del cp, rv, nz
+    bd.upload(badv)
+    P, t_fact = factor(A)
+    sh = isb.DeviceArray.from_numpy(ctx, rng.random(n))
+    rec = _ilu_record(isb, ctx, P, n)
+    for solver in ("gmres", "bicgstabl"):
+        runs = {}
+        for name, Pl in (("identity", None), ("ilu0", P)):
+            for cap in ((30, 8), (gmres_maxiter, bicgstabl_max_mv)):        # a short warm-up run, then the timed one
+                isb.lib().b200_fill(ctx._h, n, 0.0, xd._p, 0)
+                if solver == "gmres":
+                    (x, h), dt = timed(lambda: isb.gmres_(xd, A, bd, Pl=Pl, restart=30, orth_meth="cgs", maxiter=cap[0],
+                                                          initially_zero=True, log=True))
+                else:
+                    (x, h), dt = timed(lambda: isb.bicgstabl_(xd, A, bd, 2, Pl=Pl, max_mv_products=cap[1],
+                                                              initial_zero=True, r_shadow=sh, log=True))
+            runs[name] = {"iters": h.niters, "mvps": h.mvps, "converged": h.isconverged, "seconds": dt,
+                          "final_resnorm": float(h["resnorm"][-1]) if len(h["resnorm"]) else None}
+        out.append({"config": "ilu", "solver": ("gmres!(restart=30, CGS)" if solver == "gmres" else "bicgstabl!(l=2)")
+                    + ", advection_dominated(%d), default reltol" % N, "grid": N, "n": n, "nnz": int(A.nnz), **gpu,
+                    "caps": {"gmres_maxiter": gmres_maxiter, "bicgstabl_max_mv_products": bicgstabl_max_mv},
+                    "runs": runs, "ilu0_factor_seconds": t_fact, **rec,
+                    "ilu0_over_identity_time": runs["ilu0"]["seconds"] / runs["identity"]["seconds"]})
+    P.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", choices=["gmres", "lobpcg", "minres", "bicgstabl", "cg256", "widen", "general", "scattered", "cg2d",
-                                      "complex", "large"])
+                                      "complex", "large", "ilu"])
     ap.add_argument("--grid", type=int, default=256)
     ap.add_argument("--iters", type=int, default=None)
     ap.add_argument("--orth", default="cgs")
@@ -553,6 +645,10 @@ def main():
     if args.which == "complex":
         for rec in run_complex(args.grid, args.iters, args.reps):
             print(json.dumps(rec))
+        return
+    if args.which == "ilu":
+        for rec in run_ilu(args.grid):
+            print(json.dumps(rec), flush=True)
         return
     print(json.dumps(run(args.which, args.grid, args.iters, args.orth, args.reps, clocks=not args.no_clocks, solves=args.solves)))
 

@@ -653,6 +653,31 @@ B200_API int b200_lobpcg_solve_op(b200_ctx *ctx, const b200_linop *A, const b200
 B200_API int b200_lobpcg_constraint_create_b(b200_ctx *ctx, const b200_linop *B, int64_t n_local, const void *Y_dev,
                                              int64_t ldy, int nc, int capacity, int dtype, b200_lobpcg_constraint **out);
 
+/* ---------------------------------------------------------------- ILU(0) preconditioner
+ * Zero-fill incomplete LU on A's own pattern (Saad, Algorithm 10.4, IKJ order): the incomplete LU factorization that the
+ * reference's docs/src/preconditioning.md points to (IncompleteLU.jl), on the device.  L (unit diagonal, not stored) and U
+ * share one value array in A's CSR order; the factor reuses A's row offsets and column indices, so A must outlive P.
+ * The factorization and each of the two triangular solves of ldiv! are one persistent launch over the dependency levels
+ * (DESIGN.md section 22); results are bit-identical run to run and to a serial row-by-row evaluation.
+ *   _create    factors A (B200_F64 / B200_F32, square, single-GPU context, 4-byte row offsets, rows with ascending column
+ *              indices).  Checks everything before it touches data: complex operators and 8-byte row offsets ->
+ *              B200_ERR_UNSUPPORTED; a missing or zero diagonal entry of A, or a zero pivot u_ii -> B200_ERR_BREAKDOWN,
+ *              the message names the row (0-based).
+ *   _ldiv      ldiv!(y, P, x): y = U \ (L \ x), enqueued on the context's stream; x == y (ldiv!(P, x)) is allowed.  Uses
+ *              only buffers of the handle, never the context's workspace, so it may run inside a solver's callback.
+ *   _as_linop  fills a b200_linop whose apply is _ldiv: pass its address as a B200_PREC_CALLBACK preconditioner (Pl / Pr)
+ *              to cg!, gmres!, bicgstabl!, idrs!, chebyshev! or the general lobpcg.
+ *   _download  the factor values in A's CSR order (nnz values of A's dtype, host memory).
+ *   _info      levels of the forward / backward sweeps, nonzeros of the strictly lower / strictly upper part. */
+typedef struct b200_ilu0 b200_ilu0;
+B200_API int b200_ilu0_create(b200_ctx *ctx, const b200_csr *A, b200_ilu0 **out);
+B200_API int b200_ilu0_ldiv(b200_ctx *ctx, b200_ilu0 *P, const void *x_dev, void *y_dev);
+B200_API int b200_ilu0_as_linop(b200_ilu0 *P, b200_linop *out);
+B200_API int b200_ilu0_download(const b200_ilu0 *P, void *vals_host);
+B200_API int b200_ilu0_info(const b200_ilu0 *P, int *levels_forward, int *levels_backward, int64_t *nnz_lower,
+                            int64_t *nnz_upper);
+B200_API int b200_ilu0_destroy(b200_ilu0 *P);
+
 /* Test hook: the eight Rayleigh-Ritz Gram products (reference src/lobpcg.jl:586-605) of five row-major n x 16 fp32
  * device blocks X, R, AR, P, AP through one of the engine's kernels (variant 1: wgmma, variant 100 + d: wgmma with
  * d stages per accumulator hand-over, variant 2: legacy mma.sync); out_host[p * 256 + i * 16 + j], products X'AR, X'R, R'AR, X'AP, X'P, R'P, AR'P, P'AP. */

@@ -587,6 +587,30 @@ function prec_cb(P::B200LinearOperator, keep::Vector{Any})
     Precond(2, 0, Base.unsafe_convert(Ptr{Cvoid}, r))
 end
 
+# ------------------------------------------------------------------------------------------- ILU(0)
+# Zero-fill incomplete LU factored on the device (b200_ilu0_*; what IncompleteLU.jl's ilu(A, τ = 0) would give on A's
+# pattern, docs/src/preconditioning.md).  Float64 / Float32 operators; the factor reuses A's index arrays, so it keeps A.
+# As Pl / Pr it travels as B200_PREC_CALLBACK with the library's own thunk (b200_ilu0_as_linop): no Julia in the loop.
+mutable struct B200ILU0{T}
+    h::Ptr{Cvoid}
+    A::B200CSR{T}
+end
+function B200ILU0(A::B200CSR{T}) where {T<:Union{Float64,Float32}}
+    r = Ref{Ptr{Cvoid}}()
+    check(ccall((:b200_ilu0_create, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ref{Ptr{Cvoid}}), A.ctx.h, A.h, r))
+    P = B200ILU0{T}(r[], A)
+    finalizer(P -> ccall((:b200_ilu0_destroy, LIB), Cint, (Ptr{Cvoid},), P.h), P)
+end
+ldiv!(y::B200Vector{T}, P::B200ILU0{T}, x::B200Vector{T}) where {T} =
+    (check(ccall((:b200_ilu0_ldiv, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}), P.A.ctx.h, P.h, x.p, y.p)); y)
+ldiv!(P::B200ILU0, x::B200Vector) = ldiv!(x, P, x)                 # in place: the solves allow x == y
+Base.:\(P::B200ILU0{T}, x::B200Vector{T}) where {T} = ldiv!(B200Vector{T}(P.A.ctx, P.A.n), P, x)
+function prec_cb(P::B200ILU0, keep::Vector{Any})
+    r = Ref{LinOp}()
+    check(ccall((:b200_ilu0_as_linop, LIB), Cint, (Ptr{Cvoid}, Ref{LinOp}), P.h, r)); push!(keep, r, P)
+    Precond(2, 0, Base.unsafe_convert(Ptr{Cvoid}, r))
+end
+
 # gmres!(x, A, b; Pl, Pr, ...) with `mul!` / `ldiv!` callbacks  src/gmres.jl:184-194 (expand! :285-304)
 function gmres!(x::B200Vector{T}, A::Union{B200CSR{T},B200LinearOperator{T}}, b::B200Vector{T};
                 Pl = Identity(), Pr = Identity(), abstol::Real = zero(real(T)), reltol::Real = sqrt(eps(real(T))),

@@ -234,6 +234,12 @@ SIGNATURES = {
     "b200_lobpcg_solve_op": (_INT, [_P, C.POINTER(LinOp), C.POINTER(LinOp), _P, _I64, C.POINTER(LobpcgOpts), _P,
                                     C.POINTER(LobpcgResult), _P, _P]),
     "b200_lobpcg_constraint_create_b": (_INT, [_P, C.POINTER(LinOp), _I64, _P, _I64, _INT, _INT, _INT, C.POINTER(_P)]),
+    "b200_ilu0_create": (_INT, [_P, _P, C.POINTER(_P)]),
+    "b200_ilu0_ldiv": (_INT, [_P, _P, _P, _P]),
+    "b200_ilu0_as_linop": (_INT, [_P, C.POINTER(LinOp)]),
+    "b200_ilu0_download": (_INT, [_P, _P]),
+    "b200_ilu0_info": (_INT, [_P, C.POINTER(_INT), C.POINTER(_INT), C.POINTER(_I64), C.POINTER(_I64)]),
+    "b200_ilu0_destroy": (_INT, [_P]),
     "b200_dense_sygv_host": (_INT, [_INT, _P, _P, _P, _P]),
     "b200_debug_lobpcg_gram_rr": (_INT, [_P, _P, _I64, _INT, _P]),
 }

@@ -337,3 +337,64 @@ class FunctionPrec:
 
     def __init__(self, n, dtype, ldiv, ctx: Context | None = None):
         self.op = B200LinearOperator((n, n), dtype, ldiv, None, ctx)
+
+
+class ILU0Prec(FunctionPrec):
+    """Zero-fill incomplete LU of a B200CSR, factored on the device (b200_ilu0_create; Saad, Algorithm 10.4): the
+    incomplete LU the reference's docs/src/preconditioning.md recommends, as IncompleteLU.jl provides it.  Float64 and
+    Float32, square single-GPU operators with ascending column indices in every row.  A zero or missing pivot raises
+    B200Error naming the row.
+
+        ldiv_(y, x)   ldiv!(y, P, x): y = U \\ (L \\ x) on device vectors; y may be x (ldiv!(P, x))
+        factors()     (L, U) as scipy.sparse CSR matrices: L unit lower triangular, U upper triangular, A's pattern
+
+    Solvers take it where they take a FunctionPrec (cg, gmres Pl / Pr, bicgstabl, idrs, chebyshev, lobpcg): the
+    descriptor's `apply` is the library's own thunk (b200_ilu0_as_linop), so no Python runs inside the iteration.
+    The factor reuses A's index arrays, so it keeps A alive."""
+
+    def __init__(self, A: B200CSR):
+        if not isinstance(A, B200CSR):
+            raise TypeError("ILU0Prec needs a B200CSR operator")
+        self.A, self.ctx = A, A.ctx
+        self.dtype, self.n = A.dtype, A.m_local
+        self._h = C.c_void_p()
+        check(lib().b200_ilu0_create(A.ctx._h, A._h, C.byref(self._h)))
+        self.op = B200LinearOperator((self.n, self.n), self.dtype, self.ldiv_, None, self.ctx)
+        check(lib().b200_ilu0_as_linop(self._h, C.byref(self.op._c)))
+        lf, lb, nl, nu = C.c_int(), C.c_int(), C.c_int64(), C.c_int64()
+        check(lib().b200_ilu0_info(self._h, C.byref(lf), C.byref(lb), C.byref(nl), C.byref(nu)))
+        self.levels = (lf.value, lb.value)            # dependency levels of the forward and the backward solve
+        self.nnz_lower, self.nnz_upper = nl.value, nu.value
+
+    def _as_c(self, A):
+        return _lib.Precond(_lib.PREC_CALLBACK, 0, C.cast(C.pointer(self.op._c), C.c_void_p))
+
+    def ldiv_(self, y, x):
+        """ldiv!(y, P, x) on device vectors (DeviceArray or CUDA tensors), enqueued on the context's stream."""
+        check(lib().b200_ilu0_ldiv(self.ctx._h, self._h, as_device_ptr(x), as_device_ptr(y)))
+        return y
+
+    def values(self) -> np.ndarray:
+        """the factor values in A's CSR order (strictly lower part: L without its unit diagonal; the rest: U)."""
+        vals = np.empty(self.A.nnz, dtype=self.dtype)
+        check(lib().b200_ilu0_download(self._h, _vp(vals)))
+        return vals
+
+    def factors(self):
+        import scipy.sparse as sp
+        rowptr, colind, _ = self.A.download()
+        vals = self.values()
+        F = sp.csr_matrix((vals, colind, rowptr), shape=(self.n, self.n))
+        L = sp.tril(F, k=-1, format="csr") + sp.identity(self.n, dtype=self.dtype, format="csr")
+        return L.tocsr(), sp.triu(F, k=0, format="csr")
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().b200_ilu0_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
