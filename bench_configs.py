@@ -505,8 +505,9 @@ def run_large(grid=680, iters=None, reps=2, ctx=None):
     A = isb.B200CSR.laplacian(grid, 3, np.float64, ctx=ctx)
     kind, sbytes = C.c_int(), C.c_int64()
     L.b200_csr_stream_kind(A._h, C.byref(kind), C.byref(sbytes))
+    _, value_b = A.band_values
     csr_b = nnz * (V + 4) + (n + 1) * 8 + 2 * n * V           # algorithmic bytes of one SpMV (SURVEY 8d, 8-byte offsets)
-    read_b = nnz * V + sbytes.value + 2 * n * V               # what the chosen form reads: vals, its structure, x, y
+    read_b = value_b + sbytes.value + 2 * n * V               # what the chosen form reads: values, its structure, x, y
     rng = np.random.default_rng(1234321)
     b = rng.standard_normal(n)
     b /= np.linalg.norm(b)

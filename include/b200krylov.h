@@ -123,6 +123,8 @@ B200_API int b200_ctx_profile_read(b200_ctx *ctx, int slot, double *total_ms, in
  *           2 = TMA-streamed CSR kernel (when the tiles fit), 3 = band stream (when the operator has a band
  *           description and x is 16-byte aligned, else as 0).  The band stream and the CSR stream give
  *           bit-identical results.  Complex operators always take the sub-warp form
+ *   "band_values": 1 (default) = the band stream reads the 8 values of a uniform tile (every offset holds one value, see
+ *           b200_csr_band_values) instead of streaming its vals; 0 = every tile streams its vals.  Results bit-identical
  *   "snake": 1 (default) = consecutive hot kernels of a solver sweep the rows in alternating directions so
  *           that each starts on the data the previous one touched last (L2 reuse); 0 = always ascending
  *   "orth_fused": 1 (default) = orthogonalize_and_normalize! (CGS / DGKS) is ONE cooperative launch (dots, update, norm,
@@ -198,6 +200,11 @@ B200_API int b200_csr_transpose(b200_ctx *ctx, const b200_csr *A, b200_csr **out
  * vectors) that form reads per SpMV: 576 per 512-row tile for the band stream, 4*nnz + b*(rows+1) for CSR, b = 4 or 8
  * the width of the row offsets (b200_csr_index_bytes). */
 B200_API int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes);
+/* Value tables of the band stream: uniform_tiles = the operator's 512-row band tiles in which every diagonal offset holds
+ * one single value (same bit pattern); the band stream reads those 8 values per tile instead of the tile's vals (context
+ * option "band_values").  value_bytes = value bytes one SpMV reads in the form the operator got: 8 sizeof(T) per uniform
+ * tile plus sizeof(T) per nonzero of the other tiles for band operators, sizeof(T) nnz for all others (uniform_tiles 0). */
+B200_API int b200_csr_band_values(const b200_csr *A, int64_t *uniform_tiles, int64_t *value_bytes);
 /* diag(A) of the local rows into a device vector (JacobiPrec(diag(A)), reference test/cg.jl:57) */
 B200_API int b200_csr_diag(b200_ctx *ctx, const b200_csr *A, void *diag_dev);
 /* device CSR arrays back to the host (tests).  B200_ERR_UNSUPPORTED for an operator with 8-byte row offsets: use

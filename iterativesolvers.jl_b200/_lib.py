@@ -150,6 +150,7 @@ SIGNATURES = {
                              C.POINTER(_I64), C.POINTER(_I64)]),
     "b200_csr_transpose": (_INT, [_P, _P, C.POINTER(_P)]),
     "b200_csr_stream_kind": (_INT, [_P, C.POINTER(_INT), C.POINTER(_I64)]),
+    "b200_csr_band_values": (_INT, [_P, C.POINTER(_I64), C.POINTER(_I64)]),
     "b200_csr_diag": (_INT, [_P, _P, _P]),
     "b200_csr_download": (_INT, [_P, _P, _P, _P, _P]),
     "b200_csr_download64": (_INT, [_P, _P, _P, _P, _P]),

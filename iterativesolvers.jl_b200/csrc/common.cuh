@@ -98,6 +98,7 @@ struct b200_ctx {
   double *h_scalars = nullptr;   // pinned host mirror (64 doubles)
   int *h_flags = nullptr;        // pinned host flags (16 ints)
   int opt_spmv_kernel = 0;       // b200_ctx_set_option("spmv_kernel"): 0 auto, 1 sub-warp per row, 2 TMA CSR stream, 3 band stream
+  int opt_band_values = 1;       // b200_ctx_set_option("band_values"): 1 = the band stream reads uniform tiles' value tables, 0 = vals
   int opt_comm = 0;              // b200_ctx_set_option("comm"): 0 auto (peer memory if mapped), 1 NCCL, 2 peer memory
   int opt_lobpcg_mma = 1;        // b200_ctx_set_option("lobpcg_mma"): fp32 LOBPCG blocks on the tensor cores (3xTF32): 1 = Rayleigh-Ritz Gram on
                                  // wgmma (lobpcg_gram_wgmma.cuh), 2 = legacy mma.sync Gram, 0 = SIMT kernels

@@ -521,6 +521,83 @@ __global__ void __launch_bounds__(kBandBuildThreads)
   band_build(rowptr, colind, m, hdr, mask, bad);
 }
 
+// Value tables of an accepted band description (csr.cuh): one block per tile, the rows of band_build.  The i-th nonzero of
+// a row has the i-th set bit of the row's mask, so every nonzero knows its offset slot j.  A block-wide minimum and maximum
+// of the values' bit patterns per slot decide whether the tile is uniform (equal for every slot j < nb): bit patterns, not
+// ==, so that -0.0 and +0.0 or two NaN payloads are never merged.  A uniform tile gets its values in val[t*8 + j] (0 for
+// j >= nb) and pad[1] = 1; cnt[0] counts the uniform tiles and cnt[1] their nonzeros.
+template <typename T, typename I>
+__global__ void __launch_bounds__(kBandBuildThreads)
+    k_band_values(const I *__restrict__ rowptr, const T *__restrict__ vals, int64_t m, const uint8_t *__restrict__ mask,
+                  b200_band_tile *__restrict__ hdr, T *__restrict__ val, unsigned long long *__restrict__ cnt) {
+  typedef typename std::conditional<sizeof(T) == 8, unsigned long long, unsigned int>::type U;
+  constexpr int R = kBandTileRows, H = kBandBuildThreads, NB = 8;
+  __shared__ U red_lo[H / 32][NB], red_hi[H / 32][NB];
+  const U *__restrict__ bits = reinterpret_cast<const U *>(vals);
+  const int lt = threadIdx.x, lane = lt & 31, wid = lt >> 5;
+  const int64_t ntiles = (m + R - 1) / R;
+  for (int64_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int64_t r0 = t * R;
+    U lo[NB], hi[NB];
+#pragma unroll
+    for (int j = 0; j < NB; ++j) {
+      lo[j] = ~(U)0;
+      hi[j] = 0;
+    }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int64_t r = r0 + lt + q * H;
+      if (r < m) {
+        I k = rowptr[r];
+        const uint32_t mk = mask[r];
+#pragma unroll
+        for (int j = 0; j < NB; ++j)
+          if ((mk >> j) & 1u) {
+            const U b = bits[k++];
+            lo[j] = b < lo[j] ? b : lo[j];
+            hi[j] = b > hi[j] ? b : hi[j];
+          }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < NB; ++j)
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const U l = __shfl_xor_sync(0xffffffffu, lo[j], o), h = __shfl_xor_sync(0xffffffffu, hi[j], o);
+        lo[j] = l < lo[j] ? l : lo[j];
+        hi[j] = h > hi[j] ? h : hi[j];
+      }
+    if (lane == 0)
+#pragma unroll
+      for (int j = 0; j < NB; ++j) {
+        red_lo[wid][j] = lo[j];
+        red_hi[wid][j] = hi[j];
+      }
+    __syncthreads();
+    if (wid == 0) {
+      const int nb = hdr[t].nb;
+      U l = ~(U)0, h = 0;
+      if (lane < NB)
+#pragma unroll
+        for (int w = 0; w < H / 32; ++w) {
+          l = red_lo[w][lane] < l ? red_lo[w][lane] : l;
+          h = red_hi[w][lane] > h ? red_hi[w][lane] : h;
+        }
+      // every offset of the header occurs in some row of the tile, so l <= h for j < nb
+      const bool uniform = __all_sync(0xffffffffu, lane >= nb || l == h);
+      if (uniform && lane < NB) reinterpret_cast<U *>(val)[t * NB + lane] = lane < nb ? l : (U)0;
+      if (lane == 0) {
+        hdr[t].pad[1] = uniform ? 1 : 0;
+        if (uniform) {
+          atomicAdd(cnt, 1ull);
+          atomicAdd(cnt + 1, (unsigned long long)(rowptr[r0 + R < m ? r0 + R : m] - rowptr[r0]));
+        }
+      }
+    }
+    __syncthreads();   // red_lo / red_hi are rewritten for the next tile
+  }
+}
+
 template <typename T>
 __global__ void k_pack(const int *__restrict__ idx, const T *__restrict__ x, int64_t n, T *__restrict__ out) {
   for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x)
@@ -592,6 +669,32 @@ int finish_operator(b200_ctx *ctx, b200_csr *A, const b200_halo_plan *plan) {
       cudaFree(A->band_mask);
       A->band_hdr = nullptr;
       A->band_mask = nullptr;
+    } else {
+      // value tables of the uniform tiles (csr.cuh); kept only when some tile is uniform
+      B200_CUDA(cudaMalloc(&A->band_val, (size_t)8 * dtype_size(A->dtype) * ntiles));
+      unsigned long long *d_cnt = reinterpret_cast<unsigned long long *>(ctx->d_scalars + 4);
+      B200_CUDA(cudaMemsetAsync(d_cnt, 0, 2 * sizeof(unsigned long long), ctx->stream));
+      with_rowptr(A, [&](auto rp) {
+        const int grid = grid_for(ctx, ntiles, 1);
+        if (A->dtype == B200_F64)
+          k_band_values<<<grid, kBandBuildThreads, 0, ctx->stream>>>(rp, (const double *)A->vals, A->m_local, A->band_mask,
+                                                                     A->band_hdr, (double *)A->band_val, d_cnt);
+        else
+          k_band_values<<<grid, kBandBuildThreads, 0, ctx->stream>>>(rp, (const float *)A->vals, A->m_local, A->band_mask,
+                                                                     A->band_hdr, (float *)A->band_val, d_cnt);
+        return 0;
+      });
+      B200_LAUNCH_CHECK(ctx);
+      B200_CUDA(cudaMemcpyAsync(ctx->h_scalars, d_cnt, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+      B200_CUDA(cudaStreamSynchronize(ctx->stream));
+      unsigned long long h_cnt[2];
+      memcpy(h_cnt, ctx->h_scalars, sizeof(h_cnt));
+      A->band_uniform = (int64_t)h_cnt[0];
+      A->band_uniform_nnz = (int64_t)h_cnt[1];
+      if (A->band_uniform == 0) {
+        cudaFree(A->band_val);
+        A->band_val = nullptr;
+      }
     }
   }
   B200_CUDA(cudaMemsetAsync(d_max, 0, sizeof(double) * 8, ctx->stream));
@@ -1051,6 +1154,7 @@ int b200_csr_destroy(b200_csr *A) {
   cudaFree(A->halo);
   cudaFree(A->band_hdr);
   cudaFree(A->band_mask);
+  cudaFree(A->band_val);
   if (A->st_plan && A->st_plan_free) A->st_plan_free(A->st_plan);
   delete A;
   return B200_OK;
@@ -1082,6 +1186,14 @@ int b200_csr_stream_kind(const b200_csr *A, int *kind, int64_t *structure_bytes)
   }
   if (kind) *kind = k;
   if (structure_bytes) *structure_bytes = bytes;
+  return B200_OK;
+}
+
+int b200_csr_band_values(const b200_csr *A, int64_t *uniform_tiles, int64_t *value_bytes) {
+  B200_REQUIRE(A, "A is NULL");
+  const int64_t V = (int64_t)dtype_size(A->dtype);
+  if (uniform_tiles) *uniform_tiles = A->band_uniform;
+  if (value_bytes) *value_bytes = V * (A->nnz - A->band_uniform_nnz + 8 * A->band_uniform);
   return B200_OK;
 }
 

@@ -27,6 +27,9 @@ using b200::kRowptrPad;
 // vals[k0, k1) (= rowptr[r0], rowptr[r1]) in row order, and within a row in ascending offset order.  Operators with
 // 8-byte row offsets store the low 32 bits of both bounds in k0, k1 and the high 32 bits of the first in pad[0]: a tile
 // holds fewer than 2^32 nonzeros, so k1 = k0 + (uint32_t)(k1_lo - k0_lo).  pad[0] is 0 for 4-byte operators.
+// pad[1] is 1 when the tile is uniform: for every offset j < nb, all of the tile's nonzeros with offset j have the same bit
+// pattern, stored as band_val[t * 8 + j] (b200_csr); the band stream then reads those 8 values instead of vals[k0, k1).
+// pad[2..4] are 0.  As int4s: {off[0..3]}, {off[4..7]}, {nb, k0, k1, pad[0]}, {pad[1], pad[2], pad[3], pad[4]}.
 struct alignas(16) b200_band_tile {
   int off[8];   // the tile's distinct offsets col - row, ascending; entries >= nb are 0
   int nb;       // number of offsets
@@ -55,6 +58,10 @@ struct b200_csr {
   bool band_ok = false;
   struct b200_band_tile *band_hdr = nullptr;  // one 64-byte header per tile
   uint8_t *band_mask = nullptr;               // one byte per row (padded to whole tiles): bit j = the row has offset j
+  // value tables of the uniform tiles (header pad[1] == 1): 8 values of the element type per tile, indexed by tile; kept
+  // only when band_uniform > 0.  band_uniform_nnz: the nonzeros those tiles hold
+  void *band_val = nullptr;
+  int64_t band_uniform = 0, band_uniform_nnz = 0;
   // halo exchange state (world > 1)
   std::vector<int64_t> send_count, send_offset, recv_count, recv_offset;  // per peer
   int64_t n_send = 0;

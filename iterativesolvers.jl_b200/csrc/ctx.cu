@@ -245,6 +245,11 @@ int b200_ctx_set_option(b200_ctx *c, const char *name, int64_t value) {
     c->opt_spmv_kernel = (int)value;
     return B200_OK;
   }
+  if (strcmp(name, "band_values") == 0) {
+    B200_REQUIRE(value == 0 || value == 1, "band_values must be 0 or 1");
+    c->opt_band_values = (int)value;
+    return B200_OK;
+  }
   if (strcmp(name, "snake") == 0) {
     c->opt_snake = value != 0;
     return B200_OK;
@@ -289,6 +294,7 @@ int b200_ctx_get_option(const b200_ctx *c, const char *name, int64_t *value) {
   if (strcmp(name, "spmv_kernel") == 0) *value = c->opt_spmv_kernel;
   else if (strcmp(name, "comm") == 0) *value = c->opt_comm;
   else if (strcmp(name, "lobpcg_mma") == 0) *value = c->opt_lobpcg_mma;
+  else if (strcmp(name, "band_values") == 0) *value = c->opt_band_values;
   else if (strcmp(name, "snake") == 0) *value = c->opt_snake;
   else if (strcmp(name, "orth_fused") == 0) *value = c->opt_orth_fused;
   else if (strcmp(name, "pdl") == 0) *value = c->opt_pdl;

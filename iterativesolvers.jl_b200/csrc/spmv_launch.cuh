@@ -89,25 +89,36 @@ __global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
   spmv_csr_stream_kernel<T, LPR>(rowptr, colind, vals, xv, m, epi);
 }
 
-template <typename T, typename BA, typename Epi>
+template <typename T, bool VF, typename BA, typename Epi>
 __device__ __forceinline__ void spmv_band_stream_kernel(const BA &ba, const T *__restrict__ vals, const T *__restrict__ x,
                                                         int64_t nx, int64_t m, Epi &epi) {
   if (!epi.begin()) return;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ double red[kStreamThreads / 32];
-  spmv_band_tiles<T>(ba, vals, x, nx, m, epi, reinterpret_cast<BandSmem<T> *>(smem_raw), epi.rev());
+  spmv_band_tiles<T, VF>(ba, vals, x, nx, m, epi, reinterpret_cast<BandSmem<T, VF> *>(smem_raw), epi.rev());
   epi.template end<kStreamThreads>(red);
 }
 
 template <typename T, typename Epi>
 __global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
     k_spmv_band_stream(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ x, int64_t nx, int64_t m, Epi epi) {
-  spmv_band_stream_kernel<T>(ba, vals, x, nx, m, epi);
+  spmv_band_stream_kernel<T, false>(ba, vals, x, nx, m, epi);
 }
 template <typename T, typename Epi>
 __global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
     k_spmv_band_stream(BandArgs64 ba, const T *__restrict__ vals, const T *__restrict__ x, int64_t nx, int64_t m, Epi epi) {
-  spmv_band_stream_kernel<T>(ba, vals, x, nx, m, epi);
+  spmv_band_stream_kernel<T, false>(ba, vals, x, nx, m, epi);
+}
+// value-free form: every tile of the operator is uniform (BandStage, VF)
+template <typename T, typename Epi>
+__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
+    k_spmv_band_stream_vf(BandArgs ba, const T *__restrict__ vals, const T *__restrict__ x, int64_t nx, int64_t m, Epi epi) {
+  spmv_band_stream_kernel<T, true>(ba, vals, x, nx, m, epi);
+}
+template <typename T, typename Epi>
+__global__ void __launch_bounds__(kStreamThreads, kStreamCtasPerSm)
+    k_spmv_band_stream_vf(BandArgs64 ba, const T *__restrict__ vals, const T *__restrict__ x, int64_t nx, int64_t m, Epi epi) {
+  spmv_band_stream_kernel<T, true>(ba, vals, x, nx, m, epi);
 }
 
 // One launch of (A x)[row] -> epi over the local rows, in the form the operator and the option "spmv_kernel" select: the
@@ -142,11 +153,22 @@ int launch_spmv_form(b200_ctx *ctx, const b200_csr *A, const I *rowptr, const vo
     // band descriptions exist on single-GPU contexts only: x is the whole operand, n_global entries (== m for the
     // square operators of the solvers)
     typedef typename std::conditional<sizeof(I) == 8, BandArgs64, BandArgs>::type BA;
-    void (*k)(BA, const T *, const T *, int64_t, int64_t, Epi) = k_spmv_band_stream<T, Epi>;
-    const size_t smem = sizeof(BandSmem<T>);
-    B200_SMEM_ATTR_ONCE(ctx, smem, k);
-    B200_CUDA(launch_chained(chained, k, dim3(stream_grid_size(ctx, A)), dim3(kStreamThreads), smem, ctx->stream,
-                             BA{A->band_hdr, A->band_mask}, vals, (const T *)x, A->n_global, m, epi));
+    const void *tab = ctx->opt_band_values ? A->band_val : nullptr;   // null: every tile streams its vals
+    const BA ba{A->band_hdr, A->band_mask, tab};
+    const dim3 grid(stream_grid_size(ctx, A));
+    if (tab && A->band_uniform == (m + kBandTileRows - 1) / kBandTileRows) {
+      void (*k)(BA, const T *, const T *, int64_t, int64_t, Epi) = k_spmv_band_stream_vf<T, Epi>;
+      const size_t smem = sizeof(BandSmem<T, true>);
+      B200_SMEM_ATTR_ONCE(ctx, smem, k);
+      B200_CUDA(launch_chained(chained, k, grid, dim3(kStreamThreads), smem, ctx->stream, ba, vals, (const T *)x,
+                               A->n_global, m, epi));
+    } else {
+      void (*k)(BA, const T *, const T *, int64_t, int64_t, Epi) = k_spmv_band_stream<T, Epi>;
+      const size_t smem = sizeof(BandSmem<T>);
+      B200_SMEM_ATTR_ONCE(ctx, smem, k);
+      B200_CUDA(launch_chained(chained, k, grid, dim3(kStreamThreads), smem, ctx->stream, ba, vals, (const T *)x,
+                               A->n_global, m, epi));
+    }
   } else if (use_stream(ctx, A)) {
     const XView<T> xv = make_xview<T>(A, x, peer_halo);
     const size_t smem = sizeof(StreamSmem<T, I>);

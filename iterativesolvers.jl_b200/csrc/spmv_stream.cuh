@@ -262,42 +262,54 @@ __device__ __forceinline__ void spmv_stream_tiles(const I *__restrict__ rowptr, 
 // nonzero in the stage is the prefix popcount of the masks before it (one scan per group and tile), and the row sum is
 // taken over the set mask bits in ascending j = ascending column, left to right with unfused multiply and add --
 // bit-identical to the CSR stream.  Per SpMV this reads vals, 1 B/row of masks and 64 B/tile of headers instead of
-// 4 B/nonzero of colind and 4 B/row of rowptr.
+// 4 B/nonzero of colind and 4 B/row of rowptr.  A uniform tile (csr.cuh: every offset holds one value) replaces its vals
+// by its 8-value table, so an operator whose tiles are all uniform (constant-coefficient stencils) reads no vals at all.
 // ------------------------------------------------------------------------------------------------
 constexpr int kBandMax = 8;      // offsets per tile
-constexpr int kBandStages = 3;   // 3 x 66 KB (fp64) of the 227 KB of shared memory
+constexpr int kBandStages = 3;     // 3 x 66 KB (fp64) of the 227 KB of shared memory
+constexpr int kBandStagesVF = 6;   // value-free stages (every tile uniform): 6 x 33 KB (fp64)
 // the same tiles, rows per thread and CTA interleave as spmv_stream_tiles<T, 1>: every row result and every epilogue
 // partial sum (cg!'s dot(u, c)) is formed by the same thread in the same order, so the two forms are bit-identical
 static_assert(kBandTileRows == kStreamTileRows, "band tiles are the LPR == 1 stream tiles");
 
-template <typename T>
+// VF (value-free): every tile of the operator is uniform, so no stage ever receives vals; without the val region a stage
+// is half the size and the ring twice as deep, which keeps twice as many tiles' x bands landing per SM
+template <typename T, bool VF = false>
 struct alignas(128) BandStage {
-  T val[kStreamNnzCap + 8];
+  T val[VF ? 16 / sizeof(T) : kStreamNnzCap + 8];   // VF: a 16-byte stub, never read
   // band j holds x[bs_j, be_j): bs_j rounded down and be_j up to 16 bytes, so at most R + 2*(16/sizeof(T) - 1) entries
   T xb[kBandMax][kStreamTileRows + 32 / sizeof(T)];
   uint8_t mask[kStreamTileRows];
+  alignas(16) T tv[kBandMax];   // a uniform tile's value per offset (its value table), copied instead of val
 };
-template <typename T>
+template <typename T, bool VF = false>
 struct BandSmem {
-  BandStage<T> stage[kBandStages];
+  static constexpr int S = VF ? kBandStagesVF : kBandStages;
+  BandStage<T, VF> stage[S];
   // written by the producer with ordinary stores before it arrives on full[s] (never a bulk-copy target):
-  // band[s][j] = {index in xb[j] of row 0's operand, entries copied, bs_j, 0}; kofs[s] = first nonzero - first copied
-  int4 band[kBandStages][kBandMax];
-  int kofs[kBandStages];
-  int fill[kBandStages];   // number of the last fill the producer started on each stage (-1: none yet)
+  // band[s][j] = {index in xb[j] of row 0's operand, entries copied, bs_j, 0}; kofs[s] = first nonzero - first copied;
+  // uni[s] = 1: the stage holds the tile's value table in tv instead of its vals
+  int4 band[S][kBandMax];
+  int kofs[S];
+  int uni[S];
+  int fill[S];   // number of the last fill the producer started on each stage (-1: none yet)
   int scan[kStreamGroups][2][kStreamGroupThreads / 32];
-  alignas(8) unsigned long long full[kBandStages];
-  alignas(8) unsigned long long empty[kBandStages];
+  alignas(8) unsigned long long full[S];
+  alignas(8) unsigned long long empty[S];
 };
 
+// tab: the value tables of the uniform tiles (b200_csr::band_val, kBandMax values of the element type per tile), or null:
+// every tile streams its vals (the operator has no uniform tile, or the context option "band_values" is 0)
 struct BandArgs {
   const b200_band_tile *hdr;
   const uint8_t *mask;
+  const void *tab;
 };
 // the same description of an operator with 8-byte row offsets: tile bounds k0, k1 are 64-bit (b200_band_tile)
 struct BandArgs64 {
   const b200_band_tile *hdr;
   const uint8_t *mask;
+  const void *tab;
 };
 
 #ifdef __CUDACC__
@@ -318,18 +330,20 @@ __device__ __forceinline__ void bulk_g2s_plain(void *dst_smem, const void *src_g
                : "memory");
 }
 
-// Same contract as spmv_stream_tiles (LPR == 1): `x` (nx entries, 16-byte aligned) is the operand, m the rows.
-template <typename T, typename Epi, typename BA>
+// Same contract as spmv_stream_tiles (LPR == 1): `x` (nx entries, 16-byte aligned) is the operand, m the rows.  VF: every
+// tile of the operator is uniform and ba.tab is not null (BandStage).
+template <typename T, bool VF, typename Epi, typename BA>
 __device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict__ vals, const T *__restrict__ x,
-                                                int64_t nx, int64_t m, Epi &epi, BandSmem<T> *sm, bool rev = false) {
+                                                int64_t nx, int64_t m, Epi &epi, BandSmem<T, VF> *sm, bool rev = false) {
   constexpr int R = kStreamTileRows;
   constexpr int SLOTS = kStreamGroupThreads;
   constexpr int AL = 16 / (int)sizeof(T);   // elements per 16 bytes
+  constexpr int S = BandSmem<T, VF>::S;     // stages
   const int tid = threadIdx.x;
   const int64_t ntiles = (m + R - 1) / R;
   auto phys = [&](int64_t seq) -> int64_t { return rev ? ntiles - 1 - seq : seq; };
   if (tid == 0) {
-    for (int s = 0; s < kBandStages; ++s) {
+    for (int s = 0; s < S; ++s) {
       mbar_init(&sm->full[s], 1);
       mbar_init(&sm->empty[s], kStreamGroupThreads / 32);
       sm->fill[s] = -1;
@@ -345,25 +359,27 @@ __device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict
       const int64_t nxa = nx & ~(int64_t)(AL - 1);   // bands never copy past the last whole 16 bytes of x
       int64_t t = blockIdx.x;
       // the header of the next tile is fetched one iteration ahead (off the critical path)
-      int4 h0 = make_int4(0, 0, 0, 0), h1 = h0, h2 = h0;
+      int4 h0 = make_int4(0, 0, 0, 0), h1 = h0, h2 = h0, h3 = h0;
       if (t < ntiles) {
         const int4 *p = reinterpret_cast<const int4 *>(ba.hdr + phys(t));
         h0 = __ldg(p);
         h1 = __ldg(p + 1);
         h2 = __ldg(p + 2);
+        h3 = __ldg(p + 3);
       }
       for (int it = 0; t < ntiles; ++it) {
-        const int s = it % kBandStages;
-        const uint32_t ph = (uint32_t)((it / kBandStages) & 1);
+        const int s = it % S;
+        const uint32_t ph = (uint32_t)((it / S) & 1);
         const int64_t r0 = phys(t) * R;
         const int64_t rows = (r0 + R < m) ? R : m - r0;
         const int64_t tn = t + gridDim.x;
-        int4 n0 = make_int4(0, 0, 0, 0), n1 = n0, n2 = n0;
+        int4 n0 = make_int4(0, 0, 0, 0), n1 = n0, n2 = n0, n3 = n0;
         if (tn < ntiles) {
           const int4 *p = reinterpret_cast<const int4 *>(ba.hdr + phys(tn));
           n0 = __ldg(p);
           n1 = __ldg(p + 1);
           n2 = __ldg(p + 2);
+          n3 = __ldg(p + 3);
         }
         const int off[kBandMax] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
         constexpr bool K64 = std::is_same<BA, BandArgs64>::value;
@@ -377,10 +393,13 @@ __device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict
           k0 = h2.y;
           k1 = h2.z;
         }
+        // a uniform tile (header pad[1]) copies its value table instead of its vals
+        const bool uni = VF || (ba.tab != nullptr && h3.x != 0);
         mbar_wait(&sm->empty[s], ph ^ 1u);
         const K k0a = k0 & ~(K)3;
-        const uint32_t b_val = (uint32_t)(((k1 - k0a) + 3) & ~3) * (uint32_t)sizeof(T);
-        uint32_t total = b_val + (uint32_t)R;
+        const uint32_t b_val = uni ? 0u : (uint32_t)(((k1 - k0a) + 3) & ~3) * (uint32_t)sizeof(T);
+        const uint32_t b_tab = uni ? (uint32_t)(kBandMax * sizeof(T)) : 0u;
+        uint32_t total = b_val + b_tab + (uint32_t)R;
         int64_t bsj[kBandMax];
         uint32_t bb[kBandMax];
 #pragma unroll
@@ -404,11 +423,15 @@ __device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict
           sm->band[s][j] = e;
         }
         sm->kofs[s] = (int)(k0 - k0a);
-        st_release_shared(&sm->fill[s], it / kBandStages);   // see the consumers' wait
-        BandStage<T> *st = &sm->stage[s];
+        sm->uni[s] = uni ? 1 : 0;
+        st_release_shared(&sm->fill[s], it / S);   // see the consumers' wait
+        BandStage<T, VF> *st = &sm->stage[s];
         mbar_expect_tx(&sm->full[s], total);   // releases the ordinary stores above together with the arrival
         bulk_g2s(st->mask, ba.mask + r0, (uint32_t)R, &sm->full[s], pol_stream);
-        bulk_g2s(st->val, vals + k0a, b_val, &sm->full[s], pol_stream);
+        if (uni)
+          bulk_g2s(st->tv, static_cast<const T *>(ba.tab) + phys(t) * kBandMax, b_tab, &sm->full[s], pol_stream);
+        else if constexpr (!VF)
+          bulk_g2s(st->val, vals + k0a, b_val, &sm->full[s], pol_stream);
 #pragma unroll
         for (int j = 0; j < kBandMax; ++j)
           if (bb[j]) bulk_g2s_plain(st->xb[j], x + bsj[j], bb[j], &sm->full[s]);
@@ -416,6 +439,7 @@ __device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict
         h0 = n0;
         h1 = n1;
         h2 = n2;
+        h3 = n3;
       }
     }
   } else {
@@ -433,11 +457,12 @@ __device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict
     };
     T pre_next[2];
     pre_of(grp, pre_next);
+    int nscan = 0;
     for (int64_t k = grp;; k += kStreamGroups) {
       const int64_t t = (int64_t)blockIdx.x + k * gridDim.x;
       if (t >= ntiles) break;
-      const int s = (int)(k % kBandStages);
-      const uint32_t ph = (uint32_t)((k / kBandStages) & 1);
+      const int s = (int)(k % S);
+      const uint32_t ph = (uint32_t)((k / S) & 1);
       const int64_t r0 = phys(t) * R;
       const bool valid0 = r0 + slot < m, valid1 = r0 + slot + SLOTS < m;
       const T pre[2] = {pre_next[0], pre_next[1]};
@@ -448,52 +473,76 @@ __device__ __forceinline__ void spmv_band_tiles(const BA ba, const T *__restrict
       // would read a stage that is still being written and arrive on the wrong phase of empty[s], desynchronising the
       // ring until it hangs.  The producer therefore publishes the number of the fill it has started on each stage;
       // once that is n, fill n - 1 has been consumed (the producer waited for it) and fill n + 1 cannot start before
-      // this group releases the stage, so the parity wait refers to fill n alone.
-      const int fill_no = (int)(k / kBandStages);
+      // this group releases the stage, so the parity wait refers to fill n alone.  (With the 6 value-free stages a stage
+      // stays with one group; the same wait is kept, so the ring's correctness does not rest on the stage count.)
+      const int fill_no = (int)(k / S);
       while (ld_acquire_shared(&sm->fill[s]) != fill_no) __nanosleep(32);
       mbar_wait(&sm->full[s], ph);
-      const BandStage<T> *st = &sm->stage[s];
+      const BandStage<T, VF> *st = &sm->stage[s];
       const uint32_t mk0 = st->mask[slot], mk1 = st->mask[slot + SLOTS];   // 0 past the last row
-      // row starts: exclusive prefix of the popcounts over the group, both rows' counts packed in one int
-      const int own = __popc(mk0) | (__popc(mk1) << 16);
-      int inc = own;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += v;
-      }
-      int *scan = sm->scan[grp][(k / kStreamGroups) & 1];
-      if (lane == 31) scan[wig] = inc;
-      asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(kStreamGroupThreads) : "memory");
-      int before = 0, all = 0;
-#pragma unroll
-      for (int w = 0; w < kStreamGroupThreads / 32; ++w) {
-        const int v = scan[w];
-        if (w < wig) before += v;
-        all += v;
-      }
-      const int excl = before + inc - own;
-      const int kofs = sm->kofs[s];
-      int kk0 = kofs + (excl & 0xffff);
-      int kk1 = kofs + (all & 0xffff) + (excl >> 16);
       T acc[2] = {(T)0, (T)0};
-      // left-to-right, unfused multiply-add in ascending column order (see the comment above)
+      // left-to-right, unfused multiply-add in ascending column order (see the comment above).  The branch is uniform
+      // across the block; a uniform tile's value of offset j is the same bit pattern as every vals entry it stands for
+      if (VF || sm->uni[s]) {
 #pragma unroll
-      for (int j = 0; j < kBandMax; ++j) {
-        const int4 bj = sm->band[s][j];
-        if ((mk0 >> j) & 1u) {
-          const int p = slot + bj.x;
-          const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
-          if constexpr (sizeof(T) == 8) acc[0] = __dadd_rn(acc[0], __dmul_rn(st->val[kk0], xj));
-          else acc[0] = __fadd_rn(acc[0], __fmul_rn(st->val[kk0], xj));
-          ++kk0;
+        for (int j = 0; j < kBandMax; ++j) {
+          const int4 bj = sm->band[s][j];
+          const T vj = st->tv[j];
+          if ((mk0 >> j) & 1u) {
+            const int p = slot + bj.x;
+            const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
+            if constexpr (sizeof(T) == 8) acc[0] = __dadd_rn(acc[0], __dmul_rn(vj, xj));
+            else acc[0] = __fadd_rn(acc[0], __fmul_rn(vj, xj));
+          }
+          if ((mk1 >> j) & 1u) {
+            const int p = slot + SLOTS + bj.x;
+            const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
+            if constexpr (sizeof(T) == 8) acc[1] = __dadd_rn(acc[1], __dmul_rn(vj, xj));
+            else acc[1] = __fadd_rn(acc[1], __fmul_rn(vj, xj));
+          }
         }
-        if ((mk1 >> j) & 1u) {
-          const int p = slot + SLOTS + bj.x;
-          const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
-          if constexpr (sizeof(T) == 8) acc[1] = __dadd_rn(acc[1], __dmul_rn(st->val[kk1], xj));
-          else acc[1] = __fadd_rn(acc[1], __fmul_rn(st->val[kk1], xj));
-          ++kk1;
+      } else {
+        // row starts: exclusive prefix of the popcounts over the group, both rows' counts packed in one int
+        const int own = __popc(mk0) | (__popc(mk1) << 16);
+        int inc = own;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const int v = __shfl_up_sync(0xffffffffu, inc, o);
+          if (lane >= o) inc += v;
+        }
+        // the two scan buffers alternate per scan the group takes (uniform tiles take none), so a buffer is rewritten
+        // only after a bar.sync that follows every read of its previous contents
+        int *scan = sm->scan[grp][nscan++ & 1];
+        if (lane == 31) scan[wig] = inc;
+        asm volatile("bar.sync %0, %1;" ::"r"(1 + grp), "r"(kStreamGroupThreads) : "memory");
+        int before = 0, all = 0;
+#pragma unroll
+        for (int w = 0; w < kStreamGroupThreads / 32; ++w) {
+          const int v = scan[w];
+          if (w < wig) before += v;
+          all += v;
+        }
+        const int excl = before + inc - own;
+        const int kofs = sm->kofs[s];
+        int kk0 = kofs + (excl & 0xffff);
+        int kk1 = kofs + (all & 0xffff) + (excl >> 16);
+#pragma unroll
+        for (int j = 0; j < kBandMax; ++j) {
+          const int4 bj = sm->band[s][j];
+          if ((mk0 >> j) & 1u) {
+            const int p = slot + bj.x;
+            const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
+            if constexpr (sizeof(T) == 8) acc[0] = __dadd_rn(acc[0], __dmul_rn(st->val[kk0], xj));
+            else acc[0] = __fadd_rn(acc[0], __fmul_rn(st->val[kk0], xj));
+            ++kk0;
+          }
+          if ((mk1 >> j) & 1u) {
+            const int p = slot + SLOTS + bj.x;
+            const T xj = p < bj.y ? st->xb[j][p] : __ldg(x + ((int64_t)bj.z + p));
+            if constexpr (sizeof(T) == 8) acc[1] = __dadd_rn(acc[1], __dmul_rn(st->val[kk1], xj));
+            else acc[1] = __fadd_rn(acc[1], __fmul_rn(st->val[kk1], xj));
+            ++kk1;
+          }
         }
       }
       __syncwarp();

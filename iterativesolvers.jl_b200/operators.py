@@ -237,6 +237,14 @@ class B200CSR:
         check(lib().b200_csr_diag(self.ctx._h, self._h, d._p))
         return d
 
+    @property
+    def band_values(self):
+        """(uniform_tiles, value_bytes): the band tiles whose every offset holds one value, which the band stream reads as
+        8 values per tile instead of their vals, and the value bytes one SpMV reads (b200_csr_band_values)."""
+        u, vb = C.c_int64(), C.c_int64()
+        check(lib().b200_csr_band_values(self._h, C.byref(u), C.byref(vb)))
+        return u.value, vb.value
+
     def download(self):
         """(rowptr, colind, vals) of the local rows; rowptr is int32 for 4-byte operators and int64 for 8-byte ones."""
         rowptr = np.empty(self.m_local + 1, dtype=np.int64)
