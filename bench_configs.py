@@ -627,10 +627,111 @@ def run_ilu(grid=256, ctx=None, gmres_maxiter=3000, bicgstabl_max_mv=6000):
     return out
 
 
+def _amg_record(isb, ctx, P, n, applies=20):
+    """the hierarchy (rows and nonzeros per level, operator complexity), the setup split, and ms per ldiv! from CUDA
+    events over `applies` back-to-back applies.  The fine level's share is measured with torch.profiler: a V-cycle of
+    L levels is 5 (L - 1) + 1 launches in a fixed order, of which the first three and the last two are the fine level's."""
+    xd = isb.DeviceArray.from_numpy(ctx, np.random.default_rng(3).standard_normal(n))
+    yd = isb.DeviceArray(ctx, n)
+    P.ldiv_(yd, xd)
+    ctx.sync()
+    ctx.timer_start()
+    for _ in range(applies):
+        P.ldiv_(yd, xd)
+    ms = ctx.timer_stop() / applies
+    rec = {"level_rows": P.level_rows, "level_nnz": P.level_nnz, "operator_complexity": P.operator_complexity,
+           "setup_seconds": P.setup_seconds, "setup_seconds_total": sum(P.setup_seconds.values()), "ldiv_ms": ms,
+           "launches_per_ldiv": 5 * (len(P.level_rows) - 1) + 1}
+    try:
+        import torch
+        from torch.profiler import ProfilerActivity, profile
+        L = rec["launches_per_ldiv"]
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                P.ldiv_(yd, xd)
+            ctx.sync()
+            torch.cuda.synchronize()
+        ks = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA
+                     and "Memcpy" not in e.name and "Memset" not in e.name), key=lambda e: e.time_range.start)
+        if len(ks) == 5 * L and L > 1:
+            fine = total = 0.0
+            for c in range(5):
+                grp = ks[c * L:(c + 1) * L]
+                us = [e.time_range.end - e.time_range.start for e in grp]
+                fine += sum(us[:3]) + sum(us[-2:])
+                total += sum(us)
+            rec["fine_level_kernel_ms"] = fine / 5 / 1e3
+            rec["fine_level_share_of_kernel_time"] = fine / total
+    except Exception as e:                                    # the share is reported when the profiler can give it
+        rec["fine_level_share_error"] = repr(e)
+    return rec
+
+
+def run_amg(grid=256, ctx=None, gmres_maxiter=3000):
+    """the `amg` workloads: cg! (Jacobi vs smoothed-aggregation AMG) on laplace_matrix(Float64, N, 3) and gmres!(30) CGS
+    (Identity vs AMG, with a cap) on advection_dominated(N), each to the default reltol.  Setup is timed apart from the
+    solve; the solve is timed on its second run."""
+    import iterativesolvers_jl_b200 as isb
+    ctx = ctx or isb.default_context()
+    N = grid
+    n = N ** 3
+    gpu = gpu_name_power(ctx.device)
+    rng = np.random.default_rng(1234321)
+    out = []
+
+    def timed(fn):
+        ctx.sync()
+        t0 = time.perf_counter()
+        r = fn()
+        ctx.sync()
+        return r, time.perf_counter() - t0
+
+    A = isb.B200CSR.laplacian(N, 3, np.float64, ctx=ctx)
+    b = rng.standard_normal(n)
+    b /= np.linalg.norm(b)
+    bd = isb.DeviceArray.from_numpy(ctx, b)
+    xd = isb.DeviceArray.zeros(ctx, n)
+    P, t_setup = timed(lambda: isb.SmoothedAggregationPrec(A))
+    runs = {}
+    for name, Pl in (("jacobi", isb.JacobiPrec(A.diag())), ("amg", P)):
+        for rep in range(2):
+            isb.lib().b200_fill(ctx._h, n, 0.0, xd._p, 0)
+            (x, h), dt = timed(lambda: isb.cg_(xd, A, bd, Pl=Pl, initially_zero=True, log=True))
+        runs[name] = {"iters": h.niters, "converged": h.isconverged, "seconds": dt,
+                      "final_resnorm": float(h["resnorm"][-1])}
+    rec = _amg_record(isb, ctx, P, n)
+    out.append({"config": "amg", "solver": "cg!, laplace_matrix(Float64, %d, 3), default reltol" % N, "grid": N, "n": n,
+                "nnz": int(A.nnz), **gpu, "runs": runs, "amg_setup_wall_seconds": t_setup, **rec,
+                "amg_over_jacobi_solve_time": runs["amg"]["seconds"] / runs["jacobi"]["seconds"],
+                "amg_setup_plus_solve_over_jacobi": (t_setup + runs["amg"]["seconds"]) / runs["jacobi"]["seconds"]})
+    P.close()
+    del P, A
+    cp, rv, nz, shape, badv = isb.advection_dominated(N, 1000.0, base=1)
+    A = isb.B200CSR.from_csc_arrays(cp, rv, nz, shape, base=1, ctx=ctx)
+    del cp, rv, nz
+    bd.upload(badv)
+    P, t_setup = timed(lambda: isb.SmoothedAggregationPrec(A))
+    runs = {}
+    for name, Pl in (("identity", None), ("amg", P)):
+        for cap in (30, gmres_maxiter):                                     # a short warm-up run, then the timed one
+            isb.lib().b200_fill(ctx._h, n, 0.0, xd._p, 0)
+            (x, h), dt = timed(lambda: isb.gmres_(xd, A, bd, Pl=Pl, restart=30, orth_meth="cgs", maxiter=cap,
+                                                  initially_zero=True, log=True))
+        runs[name] = {"iters": h.niters, "converged": h.isconverged, "seconds": dt,
+                      "final_resnorm": float(h["resnorm"][-1]) if len(h["resnorm"]) else None}
+    rec = _amg_record(isb, ctx, P, n)
+    out.append({"config": "amg", "solver": "gmres!(restart=30, CGS), advection_dominated(%d), default reltol" % N,
+                "grid": N, "n": n, "nnz": int(A.nnz), **gpu, "caps": {"gmres_maxiter": gmres_maxiter}, "runs": runs,
+                "amg_setup_wall_seconds": t_setup, **rec,
+                "amg_over_identity_solve_time": runs["amg"]["seconds"] / runs["identity"]["seconds"]})
+    P.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("which", choices=["gmres", "lobpcg", "minres", "bicgstabl", "cg256", "widen", "general", "scattered", "cg2d",
-                                      "complex", "large", "ilu"])
+                                      "complex", "large", "ilu", "amg"])
     ap.add_argument("--grid", type=int, default=256)
     ap.add_argument("--iters", type=int, default=None)
     ap.add_argument("--orth", default="cgs")
@@ -649,6 +750,10 @@ def main():
         return
     if args.which == "ilu":
         for rec in run_ilu(args.grid):
+            print(json.dumps(rec), flush=True)
+        return
+    if args.which == "amg":
+        for rec in run_amg(args.grid):
             print(json.dumps(rec), flush=True)
         return
     print(json.dumps(run(args.which, args.grid, args.iters, args.orth, args.reps, clocks=not args.no_clocks, solves=args.solves)))

@@ -685,6 +685,43 @@ B200_API int b200_ilu0_info(const b200_ilu0 *P, int *levels_forward, int *levels
                             int64_t *nnz_upper);
 B200_API int b200_ilu0_destroy(b200_ilu0 *P);
 
+/* ---------------------------------------------------------------- smoothed-aggregation AMG preconditioner
+ * AlgebraicMultigrid.jl's `aspreconditioner(smoothed_aggregation(A))` (and pyamg's) with one candidate B = ones, the
+ * multigrid preconditioner the reference's docs/src/preconditioning.md points to, on the device (DESIGN.md section 23).
+ * The setup runs on the host in fp64: SymmetricStrength(theta), standard aggregation, fit_candidates,
+ * JacobiProlongation(4/3) with the Gershgorin bound for rho(D^-1 A), R = P', A_c = R A P, and on the coarsest level the
+ * explicit inverse (Gauss-Jordan, partial pivoting).  Each level is stored on the device in A's element type; level 0 is
+ * A itself, so A must outlive P.  ldiv! is one V-cycle from a zero initial guess with weighted-Jacobi sweeps
+ * (omega = (4/3) / rho per level); with presweeps == postsweeps it is symmetric, a valid cg! preconditioner for SPD A.
+ *   _create    builds the hierarchy (B200_F64 / B200_F32, square, single-GPU context, 4-byte row offsets, rows with
+ *              ascending column indices; opts NULL = defaults).  Checks before it touches data: complex operators and
+ *              8-byte row offsets -> B200_ERR_UNSUPPORTED; multi-GPU contexts, non-square operators, options out of
+ *              range -> B200_ERR_INVALID; a missing or zero diagonal entry -> B200_ERR_BREAKDOWN naming the row (0-based)
+ *              and level.  A coarsest level above 4096 rows -> B200_ERR_INVALID, a singular one -> B200_ERR_BREAKDOWN.
+ *   _ldiv      ldiv!(y, P, x): one V-cycle, enqueued on the context's stream; x == y (ldiv!(P, x)) is allowed.  Uses only
+ *              buffers of the handle, never the context's workspace, so it may run inside a solver's callback.
+ *   _as_linop  fills a b200_linop whose apply is _ldiv (B200_PREC_CALLBACK, as for b200_ilu0_as_linop).
+ *   _info      number of levels; rows and nonzeros of the first `cap` levels' operators; setup_seconds (5 doubles, may
+ *              be NULL): download of A, aggregation, prolongator, Galerkin products and coarse inverse, upload.
+ *   _download_level  level l's operator A_l and prolongator P_l (borrowed handles, owned by P; *P_l is NULL on the
+ *              coarsest level), the aggregate of each row of A_l (-1: isolated; not on the coarsest level) and, on the
+ *              coarsest level, A_l^-1 (rows x rows, row-major, A's element type).  Any output may be NULL. */
+typedef struct {
+  double theta;          /* strength threshold, >= 0 (default 0) */
+  int32_t max_levels;    /* >= 1 (default 10) */
+  int32_t max_coarse;    /* coarsening stops at this many rows or fewer, >= 1 (default 10) */
+  int32_t presweeps;     /* weighted-Jacobi sweeps before and after the coarse correction, >= 0 (default 1 each) */
+  int32_t postsweeps;
+} b200_amg_opts;
+typedef struct b200_amg b200_amg;
+B200_API int b200_amg_create(b200_ctx *ctx, const b200_csr *A, const b200_amg_opts *opts, b200_amg **out);
+B200_API int b200_amg_ldiv(b200_ctx *ctx, b200_amg *P, const void *x_dev, void *y_dev);
+B200_API int b200_amg_as_linop(b200_amg *P, b200_linop *out);
+B200_API int b200_amg_info(const b200_amg *P, int *levels, int64_t *rows, int64_t *nnz, int cap, double *setup_seconds);
+B200_API int b200_amg_download_level(const b200_amg *P, int level, const b200_csr **A_l, const b200_csr **P_l,
+                                     int32_t *agg, void *coarse_inv_host);
+B200_API int b200_amg_destroy(b200_amg *P);
+
 /* Test hook: the eight Rayleigh-Ritz Gram products (reference src/lobpcg.jl:586-605) of five row-major n x 16 fp32
  * device blocks X, R, AR, P, AP through one of the engine's kernels (variant 1: wgmma, variant 100 + d: wgmma with
  * d stages per accumulator hand-over, variant 2: legacy mma.sync); out_host[p * 256 + i * 16 + j], products X'AR, X'R, R'AR, X'AP, X'P, R'P, AR'P, P'AP. */

@@ -611,6 +611,39 @@ function prec_cb(P::B200ILU0, keep::Vector{Any})
     Precond(2, 0, Base.unsafe_convert(Ptr{Cvoid}, r))
 end
 
+# ------------------------------------------------------------------------------------------- smoothed-aggregation AMG
+# AlgebraicMultigrid.jl's aspreconditioner(smoothed_aggregation(A; θ, max_levels, max_coarse)) with weighted-Jacobi
+# sweeps (b200_amg_*, DESIGN section 23): the hierarchy is built on the host, the V-cycle runs on the device.  Level 0 is
+# A itself, so the preconditioner keeps A.  As Pl / Pr it travels as B200_PREC_CALLBACK with the library's own thunk.
+struct AmgOpts
+    theta::Float64
+    max_levels::Int32
+    max_coarse::Int32
+    presweeps::Int32
+    postsweeps::Int32
+end
+mutable struct B200SmoothedAggregation{T}
+    h::Ptr{Cvoid}
+    A::B200CSR{T}
+end
+function B200SmoothedAggregation(A::B200CSR{T}; θ::Real = 0.0, max_levels::Integer = 10, max_coarse::Integer = 10,
+                                 presweeps::Integer = 1, postsweeps::Integer = 1) where {T<:Union{Float64,Float32}}
+    r = Ref{Ptr{Cvoid}}()
+    o = Ref(AmgOpts(θ, max_levels, max_coarse, presweeps, postsweeps))
+    check(ccall((:b200_amg_create, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ref{AmgOpts}, Ref{Ptr{Cvoid}}), A.ctx.h, A.h, o, r))
+    P = B200SmoothedAggregation{T}(r[], A)
+    finalizer(P -> ccall((:b200_amg_destroy, LIB), Cint, (Ptr{Cvoid},), P.h), P)
+end
+ldiv!(y::B200Vector{T}, P::B200SmoothedAggregation{T}, x::B200Vector{T}) where {T} =
+    (check(ccall((:b200_amg_ldiv, LIB), Cint, (Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}), P.A.ctx.h, P.h, x.p, y.p)); y)
+ldiv!(P::B200SmoothedAggregation, x::B200Vector) = ldiv!(x, P, x)    # in place: the V-cycle allows x == y
+Base.:\(P::B200SmoothedAggregation{T}, x::B200Vector{T}) where {T} = ldiv!(B200Vector{T}(P.A.ctx, P.A.n), P, x)
+function prec_cb(P::B200SmoothedAggregation, keep::Vector{Any})
+    r = Ref{LinOp}()
+    check(ccall((:b200_amg_as_linop, LIB), Cint, (Ptr{Cvoid}, Ref{LinOp}), P.h, r)); push!(keep, r, P)
+    Precond(2, 0, Base.unsafe_convert(Ptr{Cvoid}, r))
+end
+
 # gmres!(x, A, b; Pl, Pr, ...) with `mul!` / `ldiv!` callbacks  src/gmres.jl:184-194 (expand! :285-304)
 function gmres!(x::B200Vector{T}, A::Union{B200CSR{T},B200LinearOperator{T}}, b::B200Vector{T};
                 Pl = Identity(), Pr = Identity(), abstol::Real = zero(real(T)), reltol::Real = sqrt(eps(real(T))),

@@ -13,7 +13,8 @@ The directory name contains a dot, so import it through the repo-root alias modu
 """
 from ._lib import B200Error, lib  # noqa: F401
 from .device import Context, DeviceArray, default_context, pinned_empty  # noqa: F401
-from .operators import B200CSR, B200LinearOperator, FunctionPrec, HaloPlan, Identity, ILU0Prec, JacobiPrec  # noqa: F401
+from .operators import (B200CSR, B200LinearOperator, FunctionPrec, HaloPlan, Identity, ILU0Prec, JacobiPrec,  # noqa: F401
+                        SmoothedAggregationPrec, aspreconditioner, smoothed_aggregation)
 from .history import ConvergenceHistory, niters, nprods, nrests  # noqa: F401
 from .generators import laplace_matrix, laplace_csr_slab, advection_dominated, mmread, matread  # noqa: F401
 from .solvers import (cg, cg_, chebyshev, chebyshev_, gmres, gmres_, minres, minres_, bicgstabl, bicgstabl_, lobpcg,  # noqa: F401

@@ -76,6 +76,11 @@ class IdrsOpts(C.Structure):
                 ("check_every", C.c_int32), ("reserved", C.c_int32)]
 
 
+class AmgOpts(C.Structure):
+    _fields_ = [("theta", C.c_double), ("max_levels", C.c_int32), ("max_coarse", C.c_int32), ("presweeps", C.c_int32),
+                ("postsweeps", C.c_int32)]
+
+
 APPLY_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p)   # b200_apply_fn
 
 
@@ -241,6 +246,12 @@ SIGNATURES = {
     "b200_ilu0_download": (_INT, [_P, _P]),
     "b200_ilu0_info": (_INT, [_P, C.POINTER(_INT), C.POINTER(_INT), C.POINTER(_I64), C.POINTER(_I64)]),
     "b200_ilu0_destroy": (_INT, [_P]),
+    "b200_amg_create": (_INT, [_P, _P, C.POINTER(AmgOpts), C.POINTER(_P)]),
+    "b200_amg_ldiv": (_INT, [_P, _P, _P, _P]),
+    "b200_amg_as_linop": (_INT, [_P, C.POINTER(LinOp)]),
+    "b200_amg_info": (_INT, [_P, C.POINTER(_INT), _P, _P, _INT, _P]),
+    "b200_amg_download_level": (_INT, [_P, _INT, C.POINTER(_P), C.POINTER(_P), _P, _P]),
+    "b200_amg_destroy": (_INT, [_P]),
     "b200_dense_sygv_host": (_INT, [_INT, _P, _P, _P, _P]),
     "b200_debug_lobpcg_gram_rr": (_INT, [_P, _P, _I64, _INT, _P]),
 }

@@ -406,3 +406,102 @@ class ILU0Prec(FunctionPrec):
             self.close()
         except Exception:
             pass
+
+
+def _csr_to_scipy(ctx, h, dtype):
+    """a scipy CSR copy of a device operator handle that this module does not own"""
+    import scipy.sparse as sp
+    m, n, nnz, dt = C.c_int64(), C.c_int64(), C.c_int64(), C.c_int()
+    rb, nh = C.c_int64(), C.c_int64()
+    check(lib().b200_csr_info(h, C.byref(m), C.byref(n), C.byref(nnz), C.byref(dt), C.byref(rb), C.byref(nh)))
+    rowptr = np.empty(m.value + 1, dtype=np.int64)
+    colind = np.empty(nnz.value, dtype=np.int32)
+    vals = np.empty(nnz.value, dtype=dtype)
+    check(lib().b200_csr_download64(ctx._h, h, _vp(rowptr), _vp(colind), _vp(vals)))
+    return sp.csr_matrix((vals, colind, rowptr), shape=(m.value, n.value))
+
+
+class SmoothedAggregationPrec(FunctionPrec):
+    """Smoothed-aggregation algebraic multigrid (b200_amg_create): AlgebraicMultigrid.jl's
+    `aspreconditioner(smoothed_aggregation(A))`, the multigrid preconditioner the reference's
+    docs/src/preconditioning.md recommends, with the hierarchy built on the host and the V-cycle run on the device
+    (DESIGN section 23).  Float64 and Float32, square single-GPU operators with ascending column indices in every row.
+
+        theta        strength threshold of SymmetricStrength (default 0: every off-diagonal entry is strong)
+        max_levels   at most this many levels (default 10)
+        max_coarse   coarsening stops once a level has at most this many rows (default 10)
+        presweeps, postsweeps   weighted-Jacobi sweeps around the coarse correction (default 1 each; equal counts keep
+                     the V-cycle symmetric, as cg! needs)
+
+        ldiv_(y, x)  ldiv!(y, P, x): one V-cycle from a zero initial guess on device vectors; y may be x (ldiv!(P, x))
+        levels()     per level a dict: "A" and "P" (scipy CSR; P is None on the coarsest level), "agg" (the aggregate of
+                     each row, -1 = isolated; None on the coarsest level), "inv" (the coarsest level's dense inverse)
+
+    Solvers take it where they take a FunctionPrec (cg, gmres Pl / Pr, bicgstabl, idrs, chebyshev, lobpcg): the
+    descriptor's `apply` is the library's own thunk (b200_amg_as_linop), so no Python runs inside the iteration.
+    The finest level is A itself, so the preconditioner keeps A alive."""
+
+    def __init__(self, A: B200CSR, theta=0.0, max_levels=10, max_coarse=10, presweeps=1, postsweeps=1):
+        if not isinstance(A, B200CSR):
+            raise TypeError("SmoothedAggregationPrec needs a B200CSR operator")
+        self.A, self.ctx = A, A.ctx
+        self.dtype, self.n = A.dtype, A.m_local
+        self._h = C.c_void_p()
+        opts = _lib.AmgOpts(float(theta), int(max_levels), int(max_coarse), int(presweeps), int(postsweeps))
+        check(lib().b200_amg_create(A.ctx._h, A._h, C.byref(opts), C.byref(self._h)))
+        self.op = B200LinearOperator((self.n, self.n), self.dtype, self.ldiv_, None, self.ctx)
+        check(lib().b200_amg_as_linop(self._h, C.byref(self.op._c)))
+        nl = C.c_int()
+        check(lib().b200_amg_info(self._h, C.byref(nl), None, None, 0, None))
+        rows = np.empty(nl.value, dtype=np.int64)
+        nnz = np.empty(nl.value, dtype=np.int64)
+        secs = np.empty(5, dtype=np.float64)
+        check(lib().b200_amg_info(self._h, C.byref(nl), _vp(rows), _vp(nnz), nl.value, _vp(secs)))
+        self.level_rows, self.level_nnz = [int(r) for r in rows], [int(z) for z in nnz]
+        self.operator_complexity = float(nnz.sum()) / float(nnz[0]) if nnz[0] else 1.0
+        self.setup_seconds = dict(zip(("download", "aggregation", "prolongator", "rap", "upload"), map(float, secs)))
+
+    def _as_c(self, A):
+        return _lib.Precond(_lib.PREC_CALLBACK, 0, C.cast(C.pointer(self.op._c), C.c_void_p))
+
+    def ldiv_(self, y, x):
+        """ldiv!(y, P, x) on device vectors (DeviceArray or CUDA tensors), enqueued on the context's stream."""
+        check(lib().b200_amg_ldiv(self.ctx._h, self._h, as_device_ptr(x), as_device_ptr(y)))
+        return y
+
+    def levels(self):
+        out = []
+        for l, n in enumerate(self.level_rows):
+            ha, hp = C.c_void_p(), C.c_void_p()
+            coarsest = l + 1 == len(self.level_rows)
+            agg = None if coarsest else np.empty(n, dtype=np.int32)
+            inv = np.empty((n, n), dtype=self.dtype) if coarsest else None
+            check(lib().b200_amg_download_level(self._h, l, C.byref(ha), C.byref(hp),
+                                                None if agg is None else _vp(agg), None if inv is None else _vp(inv)))
+            out.append({"A": _csr_to_scipy(self.ctx, ha, self.dtype),
+                        "P": None if coarsest else _csr_to_scipy(self.ctx, hp, self.dtype),
+                        "agg": agg, "inv": inv})
+        return out
+
+    def close(self):
+        if getattr(self, "_h", None):
+            lib().b200_amg_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def smoothed_aggregation(A: B200CSR, **kw) -> SmoothedAggregationPrec:
+    """AlgebraicMultigrid.jl's `smoothed_aggregation(A; kw...)`: the hierarchy (see SmoothedAggregationPrec)."""
+    return SmoothedAggregationPrec(A, **kw)
+
+
+def aspreconditioner(ml: SmoothedAggregationPrec) -> SmoothedAggregationPrec:
+    """AlgebraicMultigrid.jl's `aspreconditioner(ml)`: one V-cycle per ldiv!; the hierarchy already is that."""
+    if not isinstance(ml, SmoothedAggregationPrec):
+        raise TypeError("aspreconditioner takes the result of smoothed_aggregation")
+    return ml
