@@ -688,9 +688,10 @@ B200_API int b200_ilu0_destroy(b200_ilu0 *P);
 /* ---------------------------------------------------------------- smoothed-aggregation AMG preconditioner
  * AlgebraicMultigrid.jl's `aspreconditioner(smoothed_aggregation(A))` (and pyamg's) with one candidate B = ones, the
  * multigrid preconditioner the reference's docs/src/preconditioning.md points to, on the device (DESIGN.md section 23).
- * The setup runs on the host in fp64: SymmetricStrength(theta), standard aggregation, fit_candidates,
- * JacobiProlongation(4/3) with the Gershgorin bound for rho(D^-1 A), R = P', A_c = R A P, and on the coarsest level the
- * explicit inverse (Gauss-Jordan, partial pivoting).  Each level is stored on the device in A's element type; level 0 is
+ * The setup runs on the device in fp64: SymmetricStrength(theta), standard aggregation, fit_candidates,
+ * JacobiProlongation(4/3) with the Gershgorin bound for rho(D^-1 A), R = P', A_c = R (A P), and on the coarsest level the
+ * explicit inverse (Gauss-Jordan, partial pivoting, on the host: at most 4096 rows).  Every step is deterministic and
+ * gives the same bits as the serial host setup (csrc/amg_core.h) on every run.  Each level is stored on the device in A's element type; level 0 is
  * A itself, so A must outlive P.  ldiv! is one V-cycle from a zero initial guess with weighted-Jacobi sweeps
  * (omega = (4/3) / rho per level); with presweeps == postsweeps it is symmetric, a valid cg! preconditioner for SPD A.
  *   _create    builds the hierarchy (B200_F64 / B200_F32, square, single-GPU context, 4-byte row offsets, rows with
@@ -702,7 +703,8 @@ B200_API int b200_ilu0_destroy(b200_ilu0 *P);
  *              buffers of the handle, never the context's workspace, so it may run inside a solver's callback.
  *   _as_linop  fills a b200_linop whose apply is _ldiv (B200_PREC_CALLBACK, as for b200_ilu0_as_linop).
  *   _info      number of levels; rows and nonzeros of the first `cap` levels' operators; setup_seconds (5 doubles, may
- *              be NULL): download of A, aggregation, prolongator, Galerkin products and coarse inverse, upload.
+ *              be NULL): input checks, aggregation, prolongator, Galerkin products and coarse inverse, building the
+ *              level operators.
  *   _download_level  level l's operator A_l and prolongator P_l (borrowed handles, owned by P; *P_l is NULL on the
  *              coarsest level), the aggregate of each row of A_l (-1: isolated; not on the coarsest level) and, on the
  *              coarsest level, A_l^-1 (rows x rows, row-major, A's element type).  Any output may be NULL. */

@@ -613,7 +613,8 @@ end
 
 # ------------------------------------------------------------------------------------------- smoothed-aggregation AMG
 # AlgebraicMultigrid.jl's aspreconditioner(smoothed_aggregation(A; θ, max_levels, max_coarse)) with weighted-Jacobi
-# sweeps (b200_amg_*, DESIGN section 23): the hierarchy is built on the host, the V-cycle runs on the device.  Level 0 is
+# sweeps (b200_amg_*, DESIGN section 23): the hierarchy is built on the device (fp64, bit for bit the serial setup of
+# csrc/amg_core.h) and the V-cycle runs on the device.  Level 0 is
 # A itself, so the preconditioner keeps A.  As Pl / Pr it travels as B200_PREC_CALLBACK with the library's own thunk.
 struct AmgOpts
     theta::Float64

@@ -1,7 +1,8 @@
-// amg.cu -- the smoothed-aggregation AMG preconditioner on one GPU (DESIGN section 23).  The setup runs on the host
-// (amg_core.h, fp64) and uploads each level as an ordinary operator, so every level gets finish_operator's analysis: the
-// fine level of a stencil keeps its band description and value tables.  ldiv! is one V-cycle from a zero initial guess
-// (AlgebraicMultigrid.jl's aspreconditioner), every SpMV of it one launch_spmv_fused with an epilogue of this file:
+// amg.cu -- the smoothed-aggregation AMG preconditioner on one GPU (DESIGN section 23).  The setup runs on the device
+// (amg_setup.cu, fp64, bit for bit amg_core.h's serial amg_setup) and makes each level an ordinary operator, so every
+// level gets finish_operator's analysis: the fine level of a stencil keeps its band description and value tables.
+// ldiv! is one V-cycle from a zero initial guess (AlgebraicMultigrid.jl's aspreconditioner), every SpMV of it one
+// launch_spmv_fused with an epilogue of this file:
 //   SmoothEpi    y = x + w .* (b - A x)       weighted-Jacobi sweep, w = omega_s ./ diag(A) per level, ping-pong buffers
 //   ResidualEpi  r = b - A x
 //   AddEpi       y = x + P e (prolongation), or y = R r with no addend (restriction)
@@ -16,7 +17,7 @@
 #include <chrono>
 #include <memory>
 
-#include "amg_core.h"
+#include "amg_setup.cuh"
 #include "csr.cuh"
 #include "spmv_launch.cuh"
 
@@ -85,13 +86,7 @@ __global__ void __launch_bounds__(kAmgThreads) k_amg_gemv(int n, const T *__rest
   }
 }
 
-struct DevLevel {
-  const b200_csr *A = nullptr;   // level 0: the caller's operator; coarser levels: owned
-  b200_csr *P = nullptr, *R = nullptr;
-  int64_t n = 0;
-  void *w = nullptr, *b = nullptr, *x = nullptr, *u0 = nullptr, *u1 = nullptr, *inv = nullptr;
-  std::vector<int> agg;
-};
+using DevLevel = AmgDevLevel;
 
 }  // namespace
 
@@ -101,7 +96,7 @@ struct b200_amg {
   AmgOptions opts;
   std::vector<DevLevel> lev;
   std::vector<int64_t> nnz_P;
-  double seconds[5] = {0, 0, 0, 0, 0};   // download, aggregation, P, RAP + coarse inverse, upload
+  double seconds[5] = {0, 0, 0, 0, 0};   // input checks, aggregation, P, RAP + coarse inverse, level operators
   ~b200_amg() {
     if (ctx) {
       cudaSetDevice(ctx->device);
@@ -129,112 +124,29 @@ int dev_alloc(void **p, size_t bytes) {
   return B200_OK;
 }
 
-template <typename T>
-int upload_vec(void **p, const std::vector<double> &h, cudaStream_t st) {
-  std::vector<T> t(h.begin(), h.end());
-  B200_TRY(dev_alloc(p, sizeof(T) * t.size()));
-  if (!t.empty()) B200_CUDA(cudaMemcpyAsync(*p, t.data(), sizeof(T) * t.size(), cudaMemcpyHostToDevice, st));
-  B200_CUDA(cudaStreamSynchronize(st));   // t is a temporary
-  return B200_OK;
-}
-
-// a host level matrix as a device operator: square ones through the CSR slab constructor, rectangular ones (P) as the
-// CSC whose arrays are those of P' (both finish_operator'd); values rounded to T
-template <typename T>
-int upload_csr(b200_ctx *ctx, const AmgCsr &M, b200_csr **out) {
-  const int dtype = sizeof(T) == 8 ? B200_F64 : B200_F32;
-  if (M.m == M.n) {
-    std::vector<T> v(M.vals.begin(), M.vals.end());
-    std::vector<int64_t> ci(M.colind.begin(), M.colind.end());
-    return b200_csr_from_csr_slab(ctx, M.n, 0, M.m, M.rowptr.data(), ci.data(), v.data(), 8, dtype, 0, nullptr, out);
-  }
-  const AmgCsr Mt = amg_transpose(M);
-  std::vector<T> vt(Mt.vals.begin(), Mt.vals.end());
-  std::vector<int64_t> ri(Mt.colind.begin(), Mt.colind.end());
-  return b200_csr_from_csc(ctx, M.m, M.n, Mt.rowptr.data(), ri.data(), vt.data(), 8, dtype, 0, out);
-}
-
 double now_s() {
   return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
 template <typename T>
 int amg_create(b200_ctx *ctx, const b200_csr *A, const AmgOptions &o, b200_amg **out) {
-  const int64_t n = A->m_local, nnz = A->nnz;
   cudaStream_t st = ctx->stream;
   std::unique_ptr<b200_amg> H(new b200_amg());
   H->ctx = ctx;
   H->dtype = A->dtype;
   H->opts = o;
-  double t0 = now_s();
-  AmgCsr h;
-  h.m = h.n = n;
-  {
-    std::vector<int> rowptr((size_t)n + 1);
-    std::vector<T> vals((size_t)nnz);
-    h.colind.resize((size_t)nnz);
-    B200_CUDA(cudaMemcpyAsync(rowptr.data(), A->rowptr, sizeof(int) * (size_t)(n + 1), cudaMemcpyDeviceToHost, st));
-    if (nnz) {
-      B200_CUDA(cudaMemcpyAsync(h.colind.data(), A->colind, sizeof(int) * (size_t)nnz, cudaMemcpyDeviceToHost, st));
-      B200_CUDA(cudaMemcpyAsync(vals.data(), A->vals, sizeof(T) * (size_t)nnz, cudaMemcpyDeviceToHost, st));
-    }
-    B200_CUDA(cudaStreamSynchronize(st));
-    h.rowptr.assign(rowptr.begin(), rowptr.end());
-    h.vals.assign(vals.begin(), vals.end());
-  }
-  for (int64_t i = 0; i < n; ++i)
-    for (int64_t p = h.rowptr[(size_t)i] + 1; p < h.rowptr[(size_t)i + 1]; ++p)
-      B200_REQUIRE(h.colind[(size_t)p - 1] < h.colind[(size_t)p], "AMG needs rows with ascending column indices (row %lld)",
-                   (long long)i);
-  double t1 = now_s();
-  H->seconds[0] = t1 - t0;
-  std::vector<AmgLevel> levels;
-  AmgTimes tm;
-  const AmgStatus s = amg_setup(std::move(h), o, &levels, &tm, now_s);
-  if (s.code == AMG_ZERO_DIAGONAL) {
-    set_error("smoothed aggregation: zero or missing diagonal entry in row %lld (0-based) of level %d", (long long)s.row,
-              s.level);
-    return B200_ERR_BREAKDOWN;
-  }
-  if (s.code == AMG_ZERO_PIVOT) {
-    set_error("smoothed aggregation: the coarsest level (level %d) is singular: zero pivot in column %lld (0-based)",
-              s.level, (long long)s.row);
-    return B200_ERR_BREAKDOWN;
-  }
-  if (s.code == AMG_TOO_LARGE) {
-    set_error("smoothed aggregation: the coarsest level (level %d) has %lld rows, more than the %d its dense inverse "
-              "allows; raise max_levels or lower max_coarse",
-              s.level, (long long)s.row, kAmgMaxCoarsest);
-    return B200_ERR_INVALID;
-  }
-  H->seconds[1] = tm.aggregation;
-  H->seconds[2] = tm.prolongator;
-  H->seconds[3] = tm.rap;
-  t0 = now_s();
-  H->lev.resize(levels.size());
+  B200_TRY(amg_device_setup<T>(ctx, A, o, &H->lev, &H->nnz_P, H->seconds));
+  // the V-cycle's vectors
+  const double t0 = now_s();
+  H->lev[0].A = A;
   const size_t vs = sizeof(T);
-  for (size_t l = 0; l < levels.size(); ++l) {
-    AmgLevel &hl = levels[l];
+  for (size_t l = 0; l < H->lev.size(); ++l) {
     DevLevel &L = H->lev[l];
-    L.n = hl.A.m;
-    if (l == 0) {
-      L.A = A;
-    } else {
-      b200_csr *Al = nullptr;
-      B200_TRY(upload_csr<T>(ctx, hl.A, &Al));
-      L.A = Al;
-    }
-    if (l + 1 < levels.size()) {
-      B200_TRY(upload_csr<T>(ctx, hl.P, &L.P));
-      B200_TRY(b200_csr_transpose(ctx, L.P, &L.R));
-      B200_TRY(upload_vec<T>(&L.w, hl.w, st));
-      L.agg = std::move(hl.agg);
-      H->nnz_P.push_back(hl.P.nnz());
+    if (l + 1 < H->lev.size()) {
       B200_TRY(dev_alloc(&L.u0, vs * (size_t)L.n));
       B200_TRY(dev_alloc(&L.u1, vs * (size_t)L.n));
-    } else {
-      B200_TRY(upload_vec<T>(&L.inv, hl.inv, st));
-      if (l == 0) B200_TRY(dev_alloc(&L.u0, vs * (size_t)L.n));   // the copy of x when x == y
+    } else if (l == 0) {
+      B200_TRY(dev_alloc(&L.u0, vs * (size_t)L.n));   // the copy of x when x == y
     }
     if (l > 0) {
       B200_TRY(dev_alloc(&L.b, vs * (size_t)L.n));
@@ -242,7 +154,7 @@ int amg_create(b200_ctx *ctx, const b200_csr *A, const AmgOptions &o, b200_amg *
     }
   }
   B200_CUDA(cudaStreamSynchronize(st));
-  H->seconds[4] = now_s() - t0;
+  H->seconds[4] += now_s() - t0;
   *out = H.release();
   return B200_OK;
 }

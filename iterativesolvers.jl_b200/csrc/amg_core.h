@@ -1,6 +1,7 @@
 // amg_core.h -- the setup of the smoothed-aggregation AMG preconditioner (DESIGN section 23) and a serial V-cycle,
-// host C++ only.  The library (amg.cu) runs the setup and uploads the levels; the CPU tests (tests/hostsim_amg) run the
-// same setup and the serial V-cycle.  Beyond SURVEY section 8; single GPU, real element types.
+// host C++ only.  amg_setup is the serial reference: the library builds the same hierarchy, bit for bit, on the device
+// (amg_setup.cu) and calls only amg_dense_inverse from here, for the coarsest level; the CPU tests (tests/hostsim_amg)
+// run amg_setup and the serial V-cycle.  Beyond SURVEY section 8; single GPU, real element types.
 //
 // The setup is AlgebraicMultigrid.jl's / pyamg's smoothed_aggregation with one candidate (B = ones), in fp64:
 //   strength      SymmetricStrength(theta): off-diagonal a_ij is strong when |a_ij| >= theta sqrt(|a_ii a_jj|)

@@ -880,6 +880,49 @@ static int csr_from_csc_impl(b200_ctx *ctx, int64_t m, int64_t n, const IC *colp
   return status;
 }
 
+// the levels of the device AMG setup (amg_setup.cu): copies of device CSR arrays with fp64 values rounded to dtype
+int b200::csr_from_device_f64(b200_ctx *ctx, int64_t m, int64_t n, int64_t nnz, const int *rowptr, const int *colind,
+                              const double *vals, int dtype, b200_csr **out) {
+  B200_REQUIRE(dtype == B200_F64 || dtype == B200_F32, "bad dtype");
+  B200_REQUIRE(nnz >= 0 && nnz < (int64_t)INT32_MAX, "nnz=%lld does not fit int32 CSR", (long long)nnz);
+  cudaStream_t st = ctx->stream;
+  auto *A = new b200_csr();
+  A->ctx = ctx;
+  A->dtype = dtype;
+  A->m_local = A->m_global = m;
+  A->n_global = n;
+  A->nnz = nnz;
+  auto fail = [&](int s) {
+    b200_csr_destroy(A);
+    return s;
+  };
+#define CK(call)                                                                        \
+  do {                                                                                  \
+    cudaError_t _e = (call);                                                            \
+    if (_e != cudaSuccess) {                                                            \
+      set_error("%s:%d %s in `%s`", __FILE__, __LINE__, cudaGetErrorString(_e), #call); \
+      return fail(B200_ERR_CUDA);                                                       \
+    }                                                                                   \
+  } while (0)
+  CK(cudaMalloc(&A->rowptr, sizeof(int) * (m + kRowptrPad)));
+  CK(cudaMalloc(&A->colind, sizeof(int) * (nnz + kNnzPad)));
+  CK(cudaMalloc(&A->vals, dtype_size(dtype) * (nnz + kNnzPad)));
+  CK(cudaMemsetAsync(A->rowptr, 0, sizeof(int) * (m + kRowptrPad), st));
+  CK(cudaMemcpyAsync(A->rowptr, rowptr, sizeof(int) * (m + 1), cudaMemcpyDeviceToDevice, st));
+  if (nnz) {
+    CK(cudaMemcpyAsync(A->colind, colind, sizeof(int) * nnz, cudaMemcpyDeviceToDevice, st));
+    if (dtype == B200_F64) CK(cudaMemcpyAsync(A->vals, vals, sizeof(double) * nnz, cudaMemcpyDeviceToDevice, st));
+    else k_convert_vals<float, double><<<grid_for(ctx, nnz), 256, 0, st>>>(vals, nnz, (float *)A->vals);
+    ctx->launches++;
+  }
+  CK(cudaGetLastError());
+#undef CK
+  const int s = finish_operator(ctx, A, nullptr);
+  if (s != B200_OK) return fail(s);
+  *out = A;
+  return B200_OK;
+}
+
 extern "C" {
 
 int b200_csr_from_csc(b200_ctx *ctx, int64_t m, int64_t n, const void *colptr, const void *rowval, const void *nzval,

@@ -98,4 +98,8 @@ inline int real_only(const b200_csr *A, const char *entry) { return A ? real_onl
 inline bool use_peer(const b200_ctx *ctx, const b200_csr *A) {
   return ctx->world > 1 && ctx->peer_ok && A->peer_halo && ctx->opt_comm != 1;
 }
+// a single-GPU m x n operator from device CSR arrays (int32 row offsets, ascending columns, fp64 values rounded to
+// dtype), the arrays copied; the levels of the device AMG setup (amg_setup.cu)
+int csr_from_device_f64(b200_ctx *ctx, int64_t m, int64_t n, int64_t nnz, const int *rowptr, const int *colind,
+                        const double *vals, int dtype, b200_csr **out);
 }  // namespace b200

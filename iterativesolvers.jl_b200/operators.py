@@ -424,8 +424,8 @@ def _csr_to_scipy(ctx, h, dtype):
 class SmoothedAggregationPrec(FunctionPrec):
     """Smoothed-aggregation algebraic multigrid (b200_amg_create): AlgebraicMultigrid.jl's
     `aspreconditioner(smoothed_aggregation(A))`, the multigrid preconditioner the reference's
-    docs/src/preconditioning.md recommends, with the hierarchy built on the host and the V-cycle run on the device
-    (DESIGN section 23).  Float64 and Float32, square single-GPU operators with ascending column indices in every row.
+    docs/src/preconditioning.md recommends, with the hierarchy built on the device (in fp64, bit for bit the serial setup
+    of csrc/amg_core.h) and the V-cycle run on the device (DESIGN section 23).  Float64 and Float32, square single-GPU operators with ascending column indices in every row.
 
         theta        strength threshold of SymmetricStrength (default 0: every off-diagonal entry is strong)
         max_levels   at most this many levels (default 10)
@@ -434,6 +434,8 @@ class SmoothedAggregationPrec(FunctionPrec):
                      the V-cycle symmetric, as cg! needs)
 
         ldiv_(y, x)  ldiv!(y, P, x): one V-cycle from a zero initial guess on device vectors; y may be x (ldiv!(P, x))
+        setup_seconds  {"download": input checks, "aggregation", "prolongator", "rap": R A P and the coarse
+                     inverse, "upload": building the level operators}
         levels()     per level a dict: "A" and "P" (scipy CSR; P is None on the coarsest level), "agg" (the aggregate of
                      each row, -1 = isolated; None on the coarsest level), "inv" (the coarsest level's dense inverse)
 
