@@ -707,7 +707,9 @@ B200_API int b200_ilu0_destroy(b200_ilu0 *P);
  *              level operators.
  *   _download_level  level l's operator A_l and prolongator P_l (borrowed handles, owned by P; *P_l is NULL on the
  *              coarsest level), the aggregate of each row of A_l (-1: isolated; not on the coarsest level) and, on the
- *              coarsest level, A_l^-1 (rows x rows, row-major, A's element type).  Any output may be NULL. */
+ *              coarsest level, A_l^-1 (rows x rows, row-major, A's element type).  Any output may be NULL.
+ *   _pass1_launches  for the first `cap` levels, how many launches pass 1 of the level's aggregation took (a row still
+ *              undecided when its poll budget runs out makes the setup launch pass 1 again); 0 on the coarsest level. */
 typedef struct {
   double theta;          /* strength threshold, >= 0 (default 0) */
   int32_t max_levels;    /* >= 1 (default 10) */
@@ -722,6 +724,7 @@ B200_API int b200_amg_as_linop(b200_amg *P, b200_linop *out);
 B200_API int b200_amg_info(const b200_amg *P, int *levels, int64_t *rows, int64_t *nnz, int cap, double *setup_seconds);
 B200_API int b200_amg_download_level(const b200_amg *P, int level, const b200_csr **A_l, const b200_csr **P_l,
                                      int32_t *agg, void *coarse_inv_host);
+B200_API int b200_amg_pass1_launches(const b200_amg *P, int32_t *launches, int cap);
 B200_API int b200_amg_destroy(b200_amg *P);
 
 /* Test hook: the eight Rayleigh-Ritz Gram products (reference src/lobpcg.jl:586-605) of five row-major n x 16 fp32

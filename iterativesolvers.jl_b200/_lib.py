@@ -251,6 +251,7 @@ SIGNATURES = {
     "b200_amg_as_linop": (_INT, [_P, C.POINTER(LinOp)]),
     "b200_amg_info": (_INT, [_P, C.POINTER(_INT), _P, _P, _INT, _P]),
     "b200_amg_download_level": (_INT, [_P, _INT, C.POINTER(_P), C.POINTER(_P), _P, _P]),
+    "b200_amg_pass1_launches": (_INT, [_P, _P, _INT]),
     "b200_amg_destroy": (_INT, [_P]),
     "b200_dense_sygv_host": (_INT, [_INT, _P, _P, _P, _P]),
     "b200_debug_lobpcg_gram_rr": (_INT, [_P, _P, _I64, _INT, _P]),

@@ -302,6 +302,12 @@ int b200_amg_download_level(const b200_amg *P, int level, const b200_csr **A, co
   return B200_OK;
 }
 
+int b200_amg_pass1_launches(const b200_amg *P, int32_t *launches, int cap) {
+  B200_REQUIRE(P && (launches || cap <= 0), "NULL argument");
+  for (int l = 0; l < cap && l < (int)P->lev.size(); ++l) launches[l] = P->lev[(size_t)l].pass1_launches;
+  return B200_OK;
+}
+
 int b200_amg_destroy(b200_amg *P) {
   delete P;
   return B200_OK;

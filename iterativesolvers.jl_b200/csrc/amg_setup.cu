@@ -636,8 +636,8 @@ int zero_diagonal(int level, int64_t row) {
   return B200_ERR_BREAKDOWN;
 }
 
-// strength and the three passes: *x = the aggregates, *naggs their number
-int aggregate(b200_ctx *ctx, const LevelState &L, double theta, DCsr *S, Buf<int> *x, int64_t *naggs) {
+// strength and the three passes: *x = the aggregates, *naggs their number, *pass1 the launches pass 1 took
+int aggregate(b200_ctx *ctx, const LevelState &L, double theta, DCsr *S, Buf<int> *x, int64_t *naggs, int *pass1) {
   cudaStream_t st = ctx->stream;
   const int64_t n = L.n;
   S->m = S->n = n;
@@ -664,7 +664,8 @@ int aggregate(b200_ctx *ctx, const LevelState &L, double theta, DCsr *S, Buf<int
   B200_TRY(ticket.alloc(1));
   k_pass1_init<<<grid(ctx, n), kThreads, 0, st>>>(S->rows(), n, state.p);
   B200_LAUNCH_CHECK(ctx);
-  for (int left = 1; left && n;) {
+  *pass1 = 0;
+  for (int left = 1; left && n; ++*pass1) {
     B200_CUDA(cudaMemsetAsync(ticket.p, 0, sizeof(unsigned), st));
     B200_CUDA(cudaMemsetAsync(misc.p, 0, sizeof(int), st));
     k_pass1<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, st>>>(S->rows(), St.rows(), n, state.p, ticket.p,
@@ -762,7 +763,8 @@ int amg_device_setup(b200_ctx *ctx, const b200_csr *A0, const AmgOptions &o, std
     DCsr S;
     Buf<int> x;
     int64_t naggs = 0;
-    B200_TRY(aggregate(ctx, L, o.theta, &S, &x, &naggs));
+    int pass1 = 0;
+    B200_TRY(aggregate(ctx, L, o.theta, &S, &x, &naggs, &pass1));
     S.reset();
     double t1 = now_s();
     seconds[1] += t1 - t0;
@@ -819,6 +821,7 @@ int amg_device_setup(b200_ctx *ctx, const b200_csr *A0, const AmgOptions &o, std
     levels->emplace_back();
     AmgDevLevel &D = levels->back();
     D.n = n;
+    D.pass1_launches = pass1;
     {
       void *w = nullptr;
       if (cudaMalloc(&w, sizeof(T) * (size_t)(n > 0 ? n : 1)) != cudaSuccess) {

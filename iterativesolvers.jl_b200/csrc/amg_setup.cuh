@@ -13,6 +13,7 @@ struct AmgDevLevel {
   int64_t n = 0;
   void *w = nullptr, *b = nullptr, *x = nullptr, *u0 = nullptr, *u1 = nullptr, *inv = nullptr;
   std::vector<int> agg;
+  int pass1_launches = 0;   // launches of pass 1 in this level's aggregation (0 on the coarsest level)
 };
 
 // Builds the hierarchy of A (element type T, int32 row offsets, single GPU) on the device: every level's A (level 0 is

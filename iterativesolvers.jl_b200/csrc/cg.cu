@@ -170,10 +170,12 @@ __device__ __forceinline__ void wait_halo(const Comm &cm) {
 // The x update is deferred by one kernel so that u is streamed once for both updates (10 instead of 11
 // vector passes per iteration); x_k is formed from the same operands as in the reference, one launch later,
 // and k_cg_flush_x applies the last one when the loop ends.
+// s is not __restrict__: chained (PDL) after K3, which writes s->done, this kernel may only read s after pdl_wait(), and
+// a const __restrict__ s lets the compiler load s->done through the read-only path ahead of the wait.
 template <typename T>
 __global__ void __launch_bounds__(kThreads) k_cg_update_u(const T *__restrict__ r, T *__restrict__ u,
                                                           T *__restrict__ x, int64_t n,
-                                                          const CgScal *__restrict__ s, int pcg, int rev,
+                                                          const CgScal *s, int pcg, int rev,
                                                           const T *r_halo, T *__restrict__ u_halo, int n_halo,
                                                           Comm cm) {
   pdl_wait();

@@ -436,6 +436,8 @@ class SmoothedAggregationPrec(FunctionPrec):
         ldiv_(y, x)  ldiv!(y, P, x): one V-cycle from a zero initial guess on device vectors; y may be x (ldiv!(P, x))
         setup_seconds  {"download": input checks, "aggregation", "prolongator", "rap": R A P and the coarse
                      inverse, "upload": building the level operators}
+        pass1_launches  per level, the launches pass 1 of its aggregation took (more than 1 when a chain of pass-1
+                     decisions outlasts one launch's poll budget; 0 on the coarsest level)
         levels()     per level a dict: "A" and "P" (scipy CSR; P is None on the coarsest level), "agg" (the aggregate of
                      each row, -1 = isolated; None on the coarsest level), "inv" (the coarsest level's dense inverse)
 
@@ -462,6 +464,9 @@ class SmoothedAggregationPrec(FunctionPrec):
         self.level_rows, self.level_nnz = [int(r) for r in rows], [int(z) for z in nnz]
         self.operator_complexity = float(nnz.sum()) / float(nnz[0]) if nnz[0] else 1.0
         self.setup_seconds = dict(zip(("download", "aggregation", "prolongator", "rap", "upload"), map(float, secs)))
+        p1 = np.zeros(nl.value, dtype=np.int32)
+        check(lib().b200_amg_pass1_launches(self._h, _vp(p1), nl.value))
+        self.pass1_launches = [int(k) for k in p1]
 
     def _as_c(self, A):
         return _lib.Precond(_lib.PREC_CALLBACK, 0, C.cast(C.pointer(self.op._c), C.c_void_p))
